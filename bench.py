@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """bench.py -- BERT-large pretraining step throughput (training_sequences_per_second, the reference's own metric:
-run_pretraining.py:748) on N B200s of one node, synthetic data, bf16, LAMB.
+run_pretraining.py:748) on N H100s of one node, synthetic data, bf16, LAMB.
 
   python bench.py --gpus 1 --steps 8 --warmup 3                      # our arm (default)
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
@@ -39,7 +39,7 @@ def parse():
                          "step, seq 384, QA head, FusedAdam + clip (BASELINE.json configs[3])")
     ap.add_argument("--seq", type=int, default=0, help="0 = 512 (phase 2, headline) for pretrain / 384 for squad; 128 = phase 1")
     ap.add_argument("--batch", type=int, default=0, help="per-GPU micro-batch (0 = 128 @512, 512 @128 -- 65536 tokens per GPU per step; the reference ran 32 @512 / 256 @128 on 80 GB "
-                         "A100s, SURVEY.md 8d; 180 GB fits 4x that and the LAMB / allreduce cost per sequence halves again vs 64)")
+                         "A100s, SURVEY.md 8d; without a materialised score tensor 4x that fits 80 GB)")
     ap.add_argument("--max-pred", type=int, default=0)
     ap.add_argument("--no-dropout", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
@@ -47,6 +47,8 @@ def parse():
     ap.add_argument("--bucket-mb", type=int, default=100)
     ap.add_argument("--dynamic-mlm-gather", action="store_true", help="use torch.nonzero (host sync per step) like the reference instead of nonzero_static(batch*max_pred)")
     ap.add_argument("--no-reference-gpu", action="store_true", help="skip the reference-GPU leg (the unmodified reference step timed on this GPU after our arm, N=1 only)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="after the timed steps, write what the last timed step computed "
+                         "(loss, a fixed seeded sample of every updated parameter) to DIR/<name>.npy, so that two builds can be compared")
     ap.add_argument("--no-cuda-graphs", action="store_true", help="enqueue every step eagerly instead of replaying one captured CUDA graph of the whole step "
                          "(the reference driver's --cuda_graphs, run_pretraining.py:602-640,669)")
     return ap.parse_args()
@@ -57,11 +59,11 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm_gbs=d.get("hbm_gbs"), tf_burst=d.get("bf16_tflops"), tf_sustained=d.get("bf16_tflops_sustained"), source="measured")
-    return dict(hbm_gbs=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source="fallback")
+    return dict(hbm_gbs=3350.0, tf_burst=989.0, tf_sustained=989.0, source="H100 SXM data sheet (dense bf16, 700 W), not measured")
 
 
 class ClockSampler:
-    """nvidia-smi sampled every 200 ms DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampled every 200 ms DURING the timed region (clocks of the timed region)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -171,8 +173,9 @@ def reference_gpu_leg(S, steps, warmup):
     by tools/bench_reference_gpu.py in a fresh process, at the reference's own micro-batch (32 @512 / 256 @128, README.md:813-816) and at
     twice that; eager and with the reference's own --cuda_graphs.  Returns the list of result lines (or a one-line reason)."""
     tool = os.path.join(ROOT, "tools", "bench_reference_gpu.py")
-    if not os.path.exists(os.path.join(ROOT, "baseline", "_ref", "BERT", "run_pretraining.py")):
-        return {"unavailable": "baseline/_ref/BERT is not installed (python baseline/install_ref.py needs /root/reference)"}
+    from oracle.build_ref import REF_BERT
+    if not os.path.exists(os.path.join(REF_BERT, "run_pretraining.py")):
+        return {"unavailable": "no reference checkout (set DLE_REFERENCE_ROOT)"}
     base = 32 if S >= 384 else 256
     runs, out = [(base, False), (base, True), (2 * base, True)], []
     for batch, graphs in runs:
@@ -215,14 +218,14 @@ def config_dict(args, cfg, S, B, P, n):
                 "seq_len": S, "micro_batch_per_gpu": B, "global_batch": B * n, "gradient_accumulation_steps": 1,
                 "dropout": 0.0 if args.no_dropout else 0.1, "parallelism": f"dp{n}", "attention_mask": "all ones (padded to full length)",
                 "cuda_graphs": not args.no_cuda_graphs,
-                "l2_policy": "per-step working set (weights 0.67 GB + activations) exceeds the 126 MB L2; no explicit flush"}
+                "l2_policy": "per-step working set (weights 0.67 GB + activations) exceeds the 50 MB L2; no explicit flush"}
     phase = "phase-2" if S >= 384 else "phase-1"
     return {"workload": f"BERT-large {phase} pretraining step seq{S} bf16 LAMB (BASELINE.json configs[{2 if S >= 384 else 1}] per-GPU shape)",
             "seq_len": S, "micro_batch_per_gpu": B, "global_batch": B * n, "max_predictions_per_seq": P,
             "gradient_accumulation_steps": 1, "dropout": 0.0 if args.no_dropout else 0.1, "parallelism": f"dp{n}",
             "attention_mask": "all ones (padded to full length)", "mlm_gather": "torch.nonzero (sync)" if args.dynamic_mlm_gather else "nonzero_static(batch*max_pred), sync-free",
             "cuda_graphs": not (args.no_cuda_graphs or args.dynamic_mlm_gather),
-            "l2_policy": "per-step working set (weights 0.67 GB + activations >10 GB) exceeds the 126 MB L2; no explicit flush"}
+            "l2_policy": "per-step working set (weights 0.67 GB + activations >10 GB) exceeds the 50 MB L2; no explicit flush"}
 
 
 def run_reference(args):
@@ -244,6 +247,28 @@ def run_reference(args):
     print(json.dumps(line), flush=True)
 
 
+DUMP_SAMPLE = 16384          # elements kept per parameter tensor: ~23 MB of float32 for BERT-large
+
+
+def dump_outputs(out_dir, loss, model):
+    """The result of the last timed step as a caller sees it: the loss and the updated parameters.  Parameters are sampled at
+    fixed, seeded positions (the full set is 1.3 GB); every file is float32 or float64."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float(loss.detach().float().item())], dtype=np.float64))
+    rng = np.random.default_rng(1234)
+    names, parts = [], []
+    for name, p in (model.module if hasattr(model, "module") else model).named_parameters():
+        flat = p.detach().float().reshape(-1)
+        idx = np.sort(rng.choice(flat.numel(), size=min(flat.numel(), DUMP_SAMPLE), replace=False))
+        parts.append(flat[idx].cpu().numpy().astype(np.float32))
+        names.append(name)
+    np.save(os.path.join(out_dir, "params_sample.npy"), np.concatenate(parts))
+    with open(os.path.join(out_dir, "params_sample_index.json"), "w") as f:
+        json.dump({"seed": 1234, "per_tensor": DUMP_SAMPLE, "tensors": [[n, len(x)] for n, x in zip(names, parts)]}, f)
+    log(f"outputs of the last timed step written to {out_dir}")
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -256,7 +281,7 @@ def run_ours(args):
     rank = int(os.environ.get("RANK", 0))
     local = int(os.environ.get("LOCAL_RANK", 0))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py (impl=ours) needs a B200: there is no CPU path")
+        raise SystemExit("bench.py (impl=ours) needs a H100: there is no CPU path")
     torch.cuda.set_device(local)
     device = torch.device("cuda", local)
     if world > 1:
@@ -379,7 +404,7 @@ def run_ours(args):
         time.sleep(0.3)
     n0 = L.launch_count["n"]
     torch.cuda.nvtx.range_push("timed_resident")
-    torch.cuda.profiler.start()          # ncu --profile-from-start off: capture exactly the timed region (all threads)
+    torch.cuda.profiler.start()          # profilers started with capture-on-start off record exactly the timed region
     ms_res, host_res = timed(step_resident, args.steps)
     torch.cuda.profiler.stop()
     torch.cuda.nvtx.range_pop()
@@ -387,6 +412,8 @@ def run_ours(args):
     launches = (L.launch_count["n"] - n0) if launches_per_step is None else launches_per_step * args.steps
     ms_e2e, host_e2e = timed(step_e2e, args.steps)
     log(f"e2e pass: {ms_e2e / args.steps:.2f} ms/step")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, graph["loss"], model)
     final_loss = loss_host.item()
     # per-launch GEMM timing for the roofline: CUDA events cannot bracket launches inside a replayed graph, so the same step is
     # enqueued eagerly once more (same kernels, same shapes, same stream) with an event pair around every GEMM launch
@@ -405,17 +432,7 @@ def run_ours(args):
     value = T.global_throughput(B, n, args.steps, ms_res)
     e2e = T.global_throughput(B, n, args.steps, ms_e2e)
     pk = peaks()
-    traffic, traffic_src = None, None
-    tensor_active = None
-    tpath = os.path.join(ROOT, "profiles", "r02_gemm_traffic.json")
-    if os.path.exists(tpath):                     # dram__bytes_read.sum + dram__bytes_write.sum per launch, from the committed ncu capture
-        tj = json.load(open(tpath))
-        traffic, traffic_src = tj["avg_dram_traffic_bytes_per_launch"], (
-            "profiles/r02_gemm_traffic.json (ncu --set full, 12 forward GEMM launches of this command; the same 12 launches move "
-            f"{tj.get('avg_algorithmic_bytes_per_launch', 0)} algorithmic bytes on average -- algorithmic_bytes_per_launch_avg below averages ALL timed launches)")
-        ls_ = tj.get("launches", [])
-        if ls_:                                   # time-weighted sm__pipe_tensor_cycles_active of the same 12 launches (ncu, not live)
-            tensor_active = round(sum(l["tensor_active_pct"] * l["time_us"] for l in ls_) / sum(l["time_us"] for l in ls_), 1)
+    traffic, traffic_src, tensor_active = None, None, None     # per-launch DRAM traffic / tensor-pipe activity: not measured here
     by_shape = {}
     for a_, b_, f_, tag in prof:
         d = by_shape.setdefault(tag, [0, 0.0, 0.0])
@@ -436,7 +453,7 @@ def run_ours(args):
                     "ms_per_step": round(ms_e2e / args.steps, 3)},
             "host_enqueue_ms_per_step": {"resident": round(host_res, 3), "e2e": round(host_e2e, 3)},
             "gpu_launches": launches, "hbm_peak_gb": round(torch.cuda.max_memory_allocated() / 2**30, 1),
-            "roofline": {"kernel": "gemm_bf16_tcgen05_kernel (all dense projections/FFN, fwd+dgrad+wgrad)", "bound": "tensor",
+            "roofline": {"kernel": "gemm_bf16_wgmma_kernel (all dense projections/FFN, fwd+dgrad+wgrad)", "bound": "tensor",
                          "achieved": round(ach, 1), "peak": pk["tf_sustained"], "unit": "TFLOP/s", "frac": round(ach / pk["tf_sustained"], 4),
                          "peak_source": pk["source"] + " (bf16_tflops_sustained: kernel timed inside a long step)",
                          "traffic": traffic, "traffic_source": traffic_src, "tensor_pipe_active_pct_ncu": tensor_active,

@@ -1,4 +1,4 @@
-"""B200-native BERT-large pretraining hot path (NVIDIA/DeepLearningExamples PyTorch/LanguageModeling/BERT).
+"""H100-native BERT-large pretraining hot path (NVIDIA/DeepLearningExamples PyTorch/LanguageModeling/BERT).
 
 Public surface (mirrors the reference's module names):
   modeling    BertConfig, BertForPreTraining, BertModel, ... (same names / parameters / checkpoints)

@@ -92,7 +92,7 @@ def load():
         if not os.path.exists(LIB_PATH):
             raise DleError(
                 f"{LIB_PATH} not found: build it with `python -m deeplearningexamples_b200.csrc.build` "
-                "(there is no CPU/PyTorch fallback for the B200 hot path)")
+                "(there is no CPU/PyTorch fallback for the H100 hot path)")
         lib = ctypes.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(lib, name)          # AttributeError if the .so lacks a declared symbol

@@ -1,9 +1,9 @@
-"""Build libdle_b200.so in-tree with nvcc for sm_100a only.
+"""Build libdle_b200.so in-tree with nvcc for sm_90a (H100) only.
 
     python -m deeplearningexamples_b200.csrc.build [--force]
 
 Each .cu is compiled to an object (in parallel) and linked into
-deeplearningexamples_b200/libdle_b200.so.  The .so is git-ignored but travels to the GPU box.
+deeplearningexamples_b200/libdle_b200.so (git-ignored; objects go to csrc/build/).
 """
 import concurrent.futures as cf
 import os
@@ -14,10 +14,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.dirname(HERE)
 OUT = os.path.join(PKG, "libdle_b200.so")
 OBJ_DIR = os.path.join(HERE, "build")
-SOURCES = ["gemm_sm100.cu", "attention_sm100.cu", "lamb.cu", "pointwise.cu", "loss.cu"]
+SOURCES = ["gemm_sm90.cu", "attention_sm90.cu", "lamb.cu", "pointwise.cu", "loss.cu"]
 HEADERS = [os.path.join(HERE, "common.cuh"), os.path.join(os.path.dirname(PKG), "include", "dle_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -39,26 +39,6 @@ def _compile(src):
     return obj, False
 
 
-def build_variant(name, extra_flags, only=None):
-    """A/B builds of the same ABI with different compile-time switches (e.g. -DDLE_MBAR_HINT_NS=0): deeplearningexamples_b200/libdle_b200_<name>.so,
-    selected at run time with DLE_LIB_PATH (see _lib.py).  Measurement tooling only."""
-    vdir = os.path.join(OBJ_DIR, "variant_" + name)
-    os.makedirs(vdir, exist_ok=True)
-    objs = []
-    for src in SOURCES:
-        obj = os.path.join(vdir, src.replace(".cu", ".o"))
-        fl = list(extra_flags) if (only is None or src in only) else []      # `only`: the sources the switches apply to
-        r = subprocess.run([NVCC] + FLAGS + fl + ["-c", os.path.join(HERE, src), "-o", obj], capture_output=True, text=True)
-        if r.returncode != 0:
-            raise RuntimeError("nvcc failed for %s:\n%s\n%s" % (src, r.stdout, r.stderr))
-        objs.append(obj)
-    out = os.path.join(PKG, "libdle_b200_%s.so" % name)
-    r = subprocess.run([NVCC, "-shared", "-o", out] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"], capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))
-    return out
-
-
 def build(force=False, verbose=False):
     os.makedirs(OBJ_DIR, exist_ok=True)
     if force:
@@ -68,7 +48,7 @@ def build(force=False, verbose=False):
         results = list(ex.map(_compile, SOURCES))
     objs = [o for o, _ in results]
     if any(c for _, c in results) or _stale(OUT, objs):
-        cmd = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [NVCC, "-shared", "-o", OUT] + objs + ["-gencode", "arch=compute_90a,code=sm_90a"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))
@@ -79,9 +59,3 @@ def build(force=False, verbose=False):
 
 if __name__ == "__main__":
     build(force="--force" in sys.argv, verbose=True)
-    if "--variant-hint" in sys.argv:
-        print("built", build_variant("hint", ["-DDLE_MBAR_HINT_NS=0x989680"]))
-    if "--variant-gemmhint" in sys.argv:   # suspend-time hint on the GEMM kernel's mbarrier waits only
-        print("built", build_variant("gemmhint", ["-DDLE_MBAR_HINT_NS=0x989680"], only=["gemm_sm100.cu"]))
-    if "--variant-trace" in sys.argv:      # attention-backward hand-off timeline (tools/attn_trace.py)
-        print("built", build_variant("trace", ["-DDLE_ATTN_TRACE"]))

@@ -1,6 +1,6 @@
-// Shared device helpers for the sm_100a kernels: mbarrier, TMA, tcgen05/TMEM PTX wrappers,
+// Shared device helpers for the sm_90a kernels: mbarrier, TMA, wgmma and mma.sync PTX wrappers,
 // counter-based RNG for dropout, bf16 packing, tanh-GELU.  Written for
-// -gencode arch=compute_100a,code=sm_100a only.
+// -gencode arch=compute_90a,code=sm_90a only.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -67,31 +67,13 @@ __device__ __forceinline__ float2 unpack_bf16(uint32_t u) {
 }
 
 // ---------------------------------------------------------------------------------------------
-// packed fp32x2 arithmetic (Blackwell FFMA2 / FADD2 / FMUL2: one issue slot for two lanes of work) and byte permute
+// two-lane fp32 helpers (kept as pairs so the GELU / dropout code reads the same on every architecture) and byte permute
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned long long pack_f32x2(float lo, float hi) {
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ void unpack_f32x2(unsigned long long v, float& lo, float& hi) {
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
 __device__ __forceinline__ void ffma2(float& d0, float& d1, float a0, float a1, float b0, float b1, float c0, float c1) {
-    unsigned long long d;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(pack_f32x2(a0, a1)), "l"(pack_f32x2(b0, b1)), "l"(pack_f32x2(c0, c1)));
-    unpack_f32x2(d, d0, d1);
+    d0 = fmaf(a0, b0, c0); d1 = fmaf(a1, b1, c1);
 }
-__device__ __forceinline__ void fmul2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-    unsigned long long d;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(pack_f32x2(a0, a1)), "l"(pack_f32x2(b0, b1)));
-    unpack_f32x2(d, d0, d1);
-}
-__device__ __forceinline__ void fadd2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
-    unsigned long long d;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(pack_f32x2(a0, a1)), "l"(pack_f32x2(b0, b1)));
-    unpack_f32x2(d, d0, d1);
-}
+__device__ __forceinline__ void fmul2(float& d0, float& d1, float a0, float a1, float b0, float b1) { d0 = a0 * b0; d1 = a1 * b1; }
+__device__ __forceinline__ void fadd2(float& d0, float& d1, float a0, float a1, float b0, float b1) { d0 = a0 + b0; d1 = a1 + b1; }
 __device__ __forceinline__ uint32_t prmt(uint32_t a, uint32_t b, uint32_t sel) {
     uint32_t r;
     asm("prmt.b32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(sel));
@@ -111,7 +93,7 @@ __device__ __forceinline__ float gelu_tanh(float x) {
     float t = tanh_fast(c * (x + 0.044715f * x * x * x));
     return 0.5f * x * (1.0f + t);
 }
-// two lanes at a time on the packed-fp32 pipe (FMUL2 / FFMA2): 0.5 x (1 + tanh(c x (1 + 0.044715 x^2)))
+// two lanes at a time: 0.5 x (1 + tanh(c x (1 + 0.044715 x^2)))
 __device__ __forceinline__ void gelu_tanh2(float x0, float x1, float& y0, float& y1) {
     const float c0 = 0.7978845608028654f, c1 = 0.7978845608028654f * 0.044715f;
     float s0, s1, a0, a1, h0, h1;
@@ -229,22 +211,24 @@ __host__ __device__ __forceinline__ uint32_t dropout_thresh15(float p) {
     float t = p * 32768.0f + 0.5f;
     return t <= 0.f ? 0u : (t >= 32767.f ? 32767u : (uint32_t)t);
 }
-template <int ROUNDS = 7>
+// the keyed Philox block of one 32-element group, and pair-mask word i (0..15) of it
+__device__ __forceinline__ uint4 attn_dropout_block(unsigned long long seed, uint32_t stream, unsigned long long group32) {
+    return philox4x32<7>(make_uint4((uint32_t)group32, (uint32_t)(group32 >> 32), stream, 0xa77d20u),
+                         make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
+}
+__device__ __forceinline__ uint32_t attn_dropout_word(const uint4& r, int i, uint32_t k2) {
+    const int w = i >> 2, k = i & 3;
+    const uint32_t x = (w == 0) ? r.x : (w == 1) ? r.y : (w == 2) ? r.z : r.w;
+    const uint32_t C = (k == 0) ? 0x9E3779B1u : (k == 1) ? 0x85EBCA77u : (k == 2) ? 0xC2B2AE3Du : 0x27D4EB2Fu;
+    const uint32_t m = x * C;
+    const uint32_t y = ((m ^ (m >> 16)) & 0x7FFF7FFFu) + k2;
+    return prmt(y, 0u, 0xBB99u);
+}
 __device__ __forceinline__ void attn_dropout_masks16(unsigned long long seed, uint32_t stream, unsigned long long group32, uint32_t k2,
                                                      uint32_t (&mask)[16]) {
-    const uint4 r = philox4x32<ROUNDS>(make_uint4((uint32_t)group32, (uint32_t)(group32 >> 32), stream, 0xa77d20u),
-                                       make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
-    const uint32_t x[4] = {r.x, r.y, r.z, r.w};
-    const uint32_t C[4] = {0x9E3779B1u, 0x85EBCA77u, 0xC2B2AE3Du, 0x27D4EB2Fu};
+    const uint4 r = attn_dropout_block(seed, stream, group32);
 #pragma unroll
-    for (int w = 0; w < 4; ++w) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint32_t m = x[w] * C[k];
-            const uint32_t y = ((m ^ (m >> 16)) & 0x7FFF7FFFu) + k2;
-            mask[w * 4 + k] = prmt(y, 0u, 0xBB99u);
-        }
-    }
+    for (int i = 0; i < 16; ++i) mask[i] = attn_dropout_word(r, i, k2);
 }
 __host__ __device__ __forceinline__ uint32_t attn_dropout_k2(uint32_t thresh15) { return (0x8000u - thresh15) * 0x00010001u; }
 
@@ -260,16 +244,10 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
-// Wait for the phase with the given parity.  try_wait is given a suspend-time hint so that the hardware parks the waiting
-// thread until the phase flips instead of returning after the (short) default limit: ncu showed ~30 % of all executed warp
-// instructions of the attention kernels were TRYWAIT/BRA/YIELD iterations of single-lane producer / MMA-issuer waits, competing
-// for issue slots with the softmax warps of the same SM sub-partition.
+// Wait for the phase with the given parity.
 // Watchdog: a wait that has not completed after 4 s of wall clock (kernels here last milliseconds) is a protocol bug; trap so the
 // launch fails with an error instead of hanging the GPU.
-// Suspend-time hint of mbarrier.try_wait: 0 = none (the hardware's default time limit per attempt), else nanoseconds.  Round 1 used
-// 10 ms to park single-lane waiters; since the producer / MMA warps wait warp-wide (see gemm_sm100.cu) the un-hinted form measures
-// 0.6 % faster on the whole step and 3 % on attention backward (profiles/README.md, same-box A/B), so it is the default; gemm_sm100.cu
-// defines the macro before including this header because the hinted form is the faster one for its long waits.
+// Suspend-time hint of mbarrier.try_wait: 0 = none (the hardware's default time limit per attempt), else nanoseconds.
 #ifndef DLE_MBAR_HINT_NS
 #define DLE_MBAR_HINT_NS 0
 #endif
@@ -306,7 +284,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-// generic-proxy smem writes -> visible to the async proxy (TMA / tcgen05 operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------
@@ -340,81 +318,21 @@ template <int N> __device__ __forceinline__ void tma_store_wait() {
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// warp-level tensor-core MMA (mma.sync m16n8k16, bf16 in, fp32 accumulate) and ldmatrix
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
+__device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+                 : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-__device__ __forceinline__ void tmem_relinquish() {
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+__device__ __forceinline__ void ldsm_x4_trans(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+    asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+                 : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// tcgen05.commit: arrive on `bar` once all previously issued MMAs of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]; bf16 in, fp32 accumulate
-__device__ __forceinline__ void umma_bf16_ss(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-
-// Instruction descriptor for kind::f16, bf16 x bf16 -> fp32 (cute::UMMA::InstrDescriptor bit layout:
-// c_format [4,6)=1 (F32), a_format [7,10)=1 (BF16), b_format [10,13)=1, a_major bit 15, b_major bit 16
-// (0 = K-major, 1 = MN-major), n_dim [17,23) = N>>3, m_dim [24,29) = M>>4).
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, bool a_mn, bool b_mn) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn ? 1u : 0u) << 15) | ((b_mn ? 1u : 0u) << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 [0,14), LBO>>4 [16,30),
-// SBO>>4 [32,46), version=1 [46,48), layout_type [61,64) (2 = SWIZZLE_128B).
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) |
-           ((uint64_t)(sbo_bytes >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (one row per thread)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-          "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-          "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-          "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 // cp.async (LDGSTS): 16 bytes global -> shared without staging registers; groups are committed / waited per thread
 __device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void* gsrc) {

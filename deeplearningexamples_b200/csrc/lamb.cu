@@ -1,4 +1,4 @@
-// Multi-tensor LAMB for sm_100a: the whole optimizer step over every parameter tensor in three
+// Multi-tensor LAMB for sm_90a: the whole optimizer step over every parameter tensor in three
 // launches driven by a device-resident tensor/chunk table (built once), instead of the reference's
 // ~100 launches whose tensor lists travel through 4 KB kernel-argument structs.
 //
@@ -322,7 +322,7 @@ adam_apply(const LambTensorDev* __restrict__ tensors, const int2* __restrict__ c
 }
 
 static int lamb_grid(int n_chunks) {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int g = sms * 4;                                            // 4 x 512-thread CTAs resident per SM

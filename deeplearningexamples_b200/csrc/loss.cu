@@ -126,7 +126,7 @@ softmax_ce_bwd_kernel(const bf16* __restrict__ x, const long long* __restrict__ 
 using namespace dle;
 
 static int ce_grid(long long rows) {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const long long cap = (long long)sms * 8;

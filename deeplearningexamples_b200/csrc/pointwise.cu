@@ -1,4 +1,4 @@
-// HBM-bound kernels of the BERT encoder path for sm_100a: (bias+)dropout+residual+LayerNorm
+// HBM-bound kernels of the BERT encoder path for sm_90a: (bias+)dropout+residual+LayerNorm
 // forward/backward, bias+tanh-GELU, embedding gather+LayerNorm, row gathers, column sums, casts.
 // All are one-warp-per-row (or 8-element-per-thread) kernels with 128-bit global accesses and
 // warp-shuffle reductions; no shared-memory staging is needed because every byte is used once.
@@ -16,7 +16,7 @@ constexpr int LN_THREADS = LN_WARPS * 32;
 
 static int sm_count() {
     static int sms = 0;
-    if (sms == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 148; }
+    if (sms == 0) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
     return sms;
 }
 static int ln_grid(long long T) {
@@ -891,11 +891,11 @@ extern "C" int dle_cast_bf16_to_f32(const void* x, float* y, int64_t n, void* st
 }
 
 extern "C" int dle_version(char* host_buf, int host_buf_len) {
-    static const char v[] = "dle_b200 0.1 sm_100a";
+    static const char v[] = "dle_b200 0.2 sm_90a";
     if (host_buf && host_buf_len > 0) {
         int i = 0;
         for (; i < host_buf_len - 1 && v[i]; ++i) host_buf[i] = v[i];
         host_buf[i] = 0;
     }
-    return 100;
+    return 90;
 }

@@ -24,7 +24,7 @@ def _ptr(t):
 
 def _req(t, dtype=None, name="tensor"):
     if not t.is_cuda:
-        raise L.DleError(f"{name} must be a CUDA tensor (no CPU fallback in the B200 hot path)")
+        raise L.DleError(f"{name} must be a CUDA tensor (no CPU fallback in the H100 hot path)")
     if dtype is not None and t.dtype != dtype:
         raise L.DleError(f"{name} must be {dtype}, got {t.dtype}")
     return t

@@ -159,7 +159,7 @@ class FusedLAMBAMP(torch.optim.Optimizer):
                 if p.grad.is_sparse:
                     raise RuntimeError('FusedLAMB does not support sparse gradients')
                 if p.dtype not in (torch.float32, torch.bfloat16):
-                    raise RuntimeError('FusedLAMBAMP (B200) supports bf16 and fp32 parameters, got %s' % p.dtype)
+                    raise RuntimeError('FusedLAMBAMP (H100) supports bf16 and fp32 parameters, got %s' % p.dtype)
                 if not (p.is_contiguous() and p.grad.is_contiguous()):
                     raise RuntimeError('FusedLAMBAMP needs contiguous parameters and gradients')
                 state = self.state[p]
@@ -191,7 +191,7 @@ class FusedLAMBAMP(torch.optim.Optimizer):
         if not tensors:
             return None, None
         if len(grad_dtypes) != 1 or next(iter(grad_dtypes)) not in (torch.float32, torch.bfloat16):
-            raise RuntimeError('FusedLAMBAMP (B200): all gradients must share one dtype (bf16 or fp32), got %s' % grad_dtypes)
+            raise RuntimeError('FusedLAMBAMP (H100): all gradients must share one dtype (bf16 or fp32), got %s' % grad_dtypes)
         return (tensors, groups, L.DLE_DTYPE_BF16 if torch.bfloat16 in grad_dtypes else L.DLE_DTYPE_F32), tuple(sig)
 
     def _grad_signature(self):

@@ -1,4 +1,4 @@
-"""B200-native BERT: the reference's `modeling` interface over hand-written sm_100a kernels.
+"""H100-native BERT: the reference's `modeling` interface over hand-written sm_90a kernels.
 
 Mirrors PyTorch/LanguageModeling/BERT/modeling.py of NVIDIA/DeepLearningExamples: the same class names,
 constructor and forward signatures, sub-module / parameter names and shapes (= the checkpoint format:
@@ -6,7 +6,7 @@ constructor and forward signatures, sub-module / parameter names and shapes (= t
 so reference checkpoints load with load_state_dict and `torch.save(model.state_dict())` round-trips into
 the reference's run_squad.py.  What differs is underneath (ops.py / csrc/):
 
-  BertSelfAttention  modeling.py:304-384  -> one packed-QKV tcgen05 GEMM + fused attention kernel
+  BertSelfAttention  modeling.py:304-384  -> one packed-QKV wgmma GEMM + fused attention kernel
   BertSelfOutput     modeling.py:387-398  -> GEMM with bias+dropout+residual epilogue + LayerNorm kernel
   BertIntermediate   modeling.py:413-420  -> GEMM with bias+tanh-GELU epilogue
   BertOutput         modeling.py:423-434  -> as BertSelfOutput
@@ -53,7 +53,7 @@ _FUSED_ACTS = {"gelu": "gelu", "tanh": "tanh"}
 # ---------------------------------------------------------------------------------------------------
 def _require_cuda(t, what):
     if not t.is_cuda:
-        raise L.DleError(f"{what}: expected a CUDA tensor -- the B200 hot path has no CPU fallback")
+        raise L.DleError(f"{what}: expected a CUDA tensor -- the H100 hot path has no CPU fallback")
 
 
 def _tokens(x):

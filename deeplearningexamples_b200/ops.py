@@ -1,4 +1,4 @@
-"""Autograd functions composing the sm_100a kernels into the operations the reference's modules perform.
+"""Autograd functions composing the sm_90a kernels into the operations the reference's modules perform.
 
 Each Function is hand-differentiated: forward and backward call the C ABI (kernels.py) only; torch is
 used for memory, streams and the autograd graph.  Activations are bf16 [tokens, features].

@@ -85,7 +85,7 @@ class SyntheticPretrainLoader:
 
 # ---------------------------------------------------------------------------------------------------------------------
 def parse_arguments(argv=None):
-    p = argparse.ArgumentParser(description="BERT pretraining (B200-native kernels, reference argument surface)")
+    p = argparse.ArgumentParser(description="BERT pretraining (H100-native kernels, reference argument surface)")
     p.add_argument("--input_dir", default=None, type=str, help="LDDL shards directory, or 'synthetic' (default when lddl is absent)")
     p.add_argument("--config_file", default=None, type=str, required=True, help="BERT config json (bert_configs/large.json)")
     p.add_argument("--output_dir", default=None, type=str, required=True)
@@ -101,7 +101,7 @@ def parse_arguments(argv=None):
     p.add_argument("--local_rank", type=int, default=os.getenv('LOCAL_RANK', -1))
     p.add_argument("--seed", type=int, default=42)
     p.add_argument("--gradient_accumulation_steps", type=int, default=1)
-    p.add_argument("--fp16", default=False, action="store_true", help="16-bit training (bf16 on B200)")
+    p.add_argument("--fp16", default=False, action="store_true", help="16-bit training (bf16 on H100)")
     p.add_argument("--amp", default=False, action="store_true", help="alias of --fp16")
     p.add_argument("--loss_scale", type=float, default=0.0)
     p.add_argument("--log_freq", type=float, default=1.0)
@@ -145,7 +145,7 @@ def get_world_size():
 
 def setup_training(args):
     if not torch.cuda.is_available():
-        raise RuntimeError("run_pretraining needs a CUDA device: the B200 hot path has no CPU fallback")
+        raise RuntimeError("run_pretraining needs a CUDA device: the H100 hot path has no CPU fallback")
     if args.local_rank == -1:
         device = torch.device("cuda", 0)
         args.allreduce_post_accumulation = False

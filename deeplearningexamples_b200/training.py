@@ -25,7 +25,7 @@ BERT_BASE = dict(attention_probs_dropout_prob=0.1, hidden_act="gelu", hidden_dro
                  initializer_range=0.02, intermediate_size=3072, max_position_embeddings=512, num_attention_heads=12,
                  num_hidden_layers=12, type_vocab_size=2, vocab_size=30528)
 
-# training FLOPs per sequence (SURVEY.md 8d / BASELINE.md 2): 3 x forward, GEMM + attention contractions only
+# training FLOPs per sequence (SURVEY.md 8d): 3 x forward, GEMM + attention contractions only
 def train_flops_per_seq(cfg, S, P):
     L_, H, I, V = cfg["num_hidden_layers"], cfg["hidden_size"], cfg["intermediate_size"], cfg["vocab_size"]
     fwd = L_ * (6 * S * H * H + 4 * S * S * H + 2 * S * H * H + 4 * S * H * I) + (2 * P * H * H + 2 * P * H * V + 2 * H * H)

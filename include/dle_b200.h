@@ -1,4 +1,4 @@
-/* dle_b200.h -- C ABI of libdle_b200.so: hand-written sm_100a kernels for the BERT-large
+/* dle_b200.h -- C ABI of libdle_b200.so: hand-written sm_90a (H100) kernels for the BERT-large
  * pretraining hot path (NVIDIA/DeepLearningExamples, PyTorch/LanguageModeling/BERT).
  *
  * Conventions
@@ -35,11 +35,11 @@ extern "C" {
 #define DLE_DTYPE_F32 0
 #define DLE_DTYPE_BF16 1
 
-/* library / build identification: returns the compiled arch (100) and writes a version string */
+/* library / build identification: returns the compiled arch (90) and writes a version string */
 int dle_version(char* host_buf, int host_buf_len);
 
 /* ------------------------------------------------------------------------------------------
- * Dense GEMM with fused epilogue  (tcgen05.mma + TMEM + TMA)
+ * Dense GEMM with fused epilogue  (wgmma + TMA + mbarrier pipeline)
  *   D[M,N] = alpha * A[M,K] x B[N,K]^T  (+ epilogue)
  * replaces: F.linear -> cuBLAS at modeling.py:160 (LinearActivation), :345-347 (query/key/value),
  *   :395,:431 (dense), :553 (decoder) and their autograd dgrad/wgrad GEMMs; the bias+gelu
@@ -88,7 +88,7 @@ typedef struct dle_gemm_args {
 int dle_gemm_bf16(const dle_gemm_args* host_args, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * Fused multi-head self-attention (tcgen05 QK^T and PV, online softmax, in-kernel dropout);
+ * Fused multi-head self-attention (tensor-core QK^T and PV, online softmax, in-kernel dropout);
  * the [B,A,S,S] score tensor never exists in HBM.
  * replaces: BertSelfAttention.forward modeling.py:349-376 (transpose_for_scores, bmm, /sqrt(d),
  *   + mask, softmax, dropout, bmm, transpose+contiguous) and its autograd backward.
@@ -102,7 +102,7 @@ int dle_gemm_bf16(const dle_gemm_args* host_args, void* stream);
 int dle_attn_fwd(const void* qkv, const float* mask, void* ctx, float* lse, int32_t B, int32_t S, int32_t A,
                  int32_t seq_first, float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, void* stream);
 /* delta_ws: fp32 workspace [B, A, S] (row dots of dO and O); dqkv: bf16 [B*S, 3*A*64], fully overwritten (dQ, dK and dV are
- * accumulated in tensor memory: no atomics, bitwise reproducible);
+ * each accumulated on chip by exactly one CTA: no atomics, bitwise reproducible);
  * dbias_qkv: fp32 [3*A*64] or NULL: += column sums of dqkv (the q/k/v bias gradients), must be zeroed by the caller */
 int dle_attn_bwd(const void* qkv, const float* mask, const void* ctx, const void* dctx, const float* lse,
                  void* dqkv, float* delta_ws, float* dbias_qkv, int32_t B, int32_t S, int32_t A, int32_t seq_first, float dropout_p,

@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE ONLY (see oracle/__init__.py).
 
-Follows /root/reference/PyTorch/LanguageModeling/BERT/lamb_amp_opt/fused_lamb/fused_lamb.py:130-260
+Follows PyTorch/LanguageModeling/BERT/lamb_amp_opt/fused_lamb/fused_lamb.py:130-260
 and schedulers.py:109-136 (PolyWarmUpScheduler).  numpy float32 arrays in, updated in place.
 """
 import ctypes
@@ -164,7 +164,7 @@ def poly_warmup_lr(step_after, total_steps, warmup, base_lr, degree=0.5):
 def adam_step_numpy(groups, *, scale=1.0, max_grad_norm=0.0, clip_eps=1e-6, adam_w_mode=True):
     """CPU oracle for the SQuAD optimizer step: GradientClipper (run_squad.py:716-724: coef = max/(norm + 1e-6), applied when
     < 1) followed by Adam/AdamW as apex.optimizers.FusedAdam is called at run_squad.py:973-975 (bias_correction=False there).
-    apex is not vendored in /root/reference (unpinned): the arithmetic is the published Adam/AdamW update, pinned against
+    apex is not vendored in the reference (unpinned): the arithmetic is the published Adam/AdamW update, pinned against
     torch.optim.AdamW in tests/test_lamb_oracle.py.  fp32 element math, double norm."""
     f = np.float32
     tot = sum(float(np.sum(a.astype(np.float64) ** 2)) for g in groups for a in g["grads"])

@@ -1,7 +1,7 @@
-"""`import modeling` for the UNMODIFIED reference scripts: the B200-native mirror under the reference's module name.
+"""`import modeling` for the UNMODIFIED reference scripts: the H100-native mirror under the reference's module name.
 
 Put this directory on sys.path ahead of the reference tree (tools/run_reference_driver.py does) and
-PyTorch/LanguageModeling/BERT/run_pretraining.py drives the sm_100a kernels without an edited line:
+PyTorch/LanguageModeling/BERT/run_pretraining.py drives the sm_90a kernels without an edited line:
   * modeling.BertConfig / BertForPreTraining(config, sequence_output_is_dense=...) / .checkpoint_activations(...) -- same surface;
   * `model.half()` (run_pretraining.py:416-417) selects bfloat16 (modeling.BertPreTrainedModel.half);
   * pass the driver's own `--disable_jit_fusions` (custom autograd Functions are not TorchScript-able, SURVEY.md 8b);

@@ -4,5 +4,5 @@ try:
     import fused_lamb_CUDA as _ext
     multi_tensor_l2norm = _ext.multi_tensor_l2norm
     multi_tensor_lamb = _ext.multi_tensor_lamb
-except ImportError:                                        # B200 arm: the optimizer shim never touches these
+except ImportError:                                        # H100 arm: the optimizer shim never touches these
     multi_tensor_l2norm = multi_tensor_lamb = None

@@ -3,4 +3,4 @@ is absent offline.  Any attribute access fails loudly."""
 
 
 def __getattr__(name):
-    raise ImportError("h5py stand-in: the HDF5 data path is not part of the B200 hot path (attribute %r requested)" % name)
+    raise ImportError("h5py stand-in: the HDF5 data path is not part of the H100 hot path (attribute %r requested)" % name)

@@ -12,7 +12,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run through gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 GPU")
 
 
 @pytest.fixture(scope="session")

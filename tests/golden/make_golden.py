@@ -1,6 +1,6 @@
 """Generate golden vectors by running the UNMODIFIED reference modeling.py (imported from
-/root/reference, authoring container only) on seeded inputs.  Commit the outputs; the GPU
-box has no /root/reference.
+a reference checkout named by $DLE_REFERENCE_ROOT) on seeded inputs.  Commit the outputs; the tests
+themselves never need the reference.
 
     python tests/golden/make_golden.py
 
@@ -28,7 +28,7 @@ import torch.nn.functional as F
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
-REF = "/root/reference/PyTorch/LanguageModeling/BERT"
+REF = os.path.join(os.environ.get("DLE_REFERENCE_ROOT", ""), "PyTorch/LanguageModeling/BERT")
 sys.path.insert(0, ROOT)
 
 

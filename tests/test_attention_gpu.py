@@ -1,4 +1,4 @@
-"""GPU parity: fused tcgen05 attention fwd/bwd vs a plain torch fp32 restatement of
+"""GPU parity: fused attention fwd/bwd vs a plain torch fp32 restatement of
 BertSelfAttention (modeling.py:349-376) on the same bf16 inputs."""
 import math
 

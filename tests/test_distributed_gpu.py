@@ -1,11 +1,11 @@
-"""2-rank NCCL equivalence of the PRODUCT path (BASELINE.md 3.C, SURVEY.md 8e): one optimizer step of the CUDA model under torch DDP on
+"""2-rank NCCL equivalence of the PRODUCT path (SURVEY.md 8e): one optimizer step of the CUDA model under torch DDP on
 two GPUs, each rank on its half of a batch, must equal the 1-rank step on the concatenated batch (dropout off).
 
 Every per-token computation is identical in both runs (sequences never interact); only the token-dimension reductions (weight /
 bias / LayerNorm gradients, the loss mean) are split across ranks.  With fp32 parameters those reductions are fp32 sums of identical
 bf16 products in a different order, so gradients, LAMB moments and parameters agree to ~1e-6 (bar: 1e-5, the north_star's LAMB
 tolerance).  With bf16 parameters each rank's gradient is rounded to bf16 before the allreduce, so the bar is the bf16 one.
-Skipped when fewer than two GPUs are visible (gpurun --gpus 2 runs it)."""
+Skipped when fewer than two GPUs are visible."""
 import os
 import socket
 
@@ -74,7 +74,7 @@ def _worker(rank, world, port, dtype_name, out_path):
 @pytest.mark.parametrize("dtype_name,tol", [("float32", 1e-5), ("bfloat16", 2e-2)])
 def test_two_rank_ddp_step_equals_one_rank_step_on_concatenated_batch(tmp_path, dtype_name, tol):
     if torch.cuda.device_count() < 2:
-        pytest.skip("needs 2 GPUs (gpurun --gpus 2)")
+        pytest.skip("needs 2 GPUs")
     import torch.multiprocessing as mp
     from deeplearningexamples_b200 import training as T
     out = str(tmp_path / "rank0.pt")

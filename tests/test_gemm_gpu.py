@@ -1,4 +1,4 @@
-"""GPU parity: tcgen05 GEMM (all operand layouts and epilogues) vs a plain torch fp32 reference of the
+"""GPU parity: wgmma GEMM (all operand layouts and epilogues) vs a plain torch fp32 reference of the
 same op on the same bf16 inputs.  Tolerance: bf16 output rounding (rel 2^-8) + fp32 accumulation order."""
 import pytest
 import torch
@@ -97,8 +97,8 @@ def test_epilogue_dgelu_and_add():
 
 @pytest.mark.parametrize("M,N,K", [(130, 264, 72), (1000, 776, 320), (4096, 4096, 1024)])
 def test_epilogue_dgelu_ragged_and_wide(M, N, K):
-    """The gelu'(u) epilogue runs on the 16-epilogue-warp instance of the kernel (four warps per TMEM lane quarter, 64 columns each, 3-stage
-    ring): partial row tiles, a last column tile with 8 valid columns, and the full FFN width, with the column sums."""
+    """The gelu'(u) epilogue on the 256-wide tile: partial row tiles, a last column tile with 8 valid columns, and the full FFN width,
+    with the column sums."""
     k, L = _k()
     a, w, u = _rand((M, K), seed=50), _rand((K, N), 0.05, seed=51), _rand((M, N), 1.5, seed=52)
     cs = torch.zeros(N, device="cuda")
@@ -188,7 +188,7 @@ def test_epilogue_column_sums_of_output():
 def test_epilogues_many_tiles_per_cta(N, tile_n):
     """Persistent-kernel state that only shows with several tiles per CTA (the encoder shapes run 14+): the bias slice is staged one
     tile ahead and rotates over three shared-memory slots, and the residual / pre-activation operand of a tile's first chunk is
-    prefetched by cp.async from the previous tile's last chunk.  16384 x N output = 512 tiles on 148 CTAs, non-zero bias that differs
+    prefetched by cp.async from the previous tile's last chunk.  16384 x N output = 512 tiles on 132 CTAs, non-zero bias that differs
     per column tile, every epilogue that takes a bias or an aux operand, against fp32 torch."""
     k, L = _k()
     M, K = 16384, 256

@@ -1,4 +1,4 @@
-"""GPU parity of the whole boundary: deeplearningexamples_b200.modeling.BertForPreTraining (bf16, sm_100a kernels)
+"""GPU parity of the whole boundary: deeplearningexamples_b200.modeling.BertForPreTraining (bf16, sm_90a kernels)
 vs (a) golden vectors produced by the reference's modeling.py (tests/golden/bert_small_golden.pt) and (b) the CPU
 oracle run on the same weights, for forward logits/loss and every parameter gradient.
 

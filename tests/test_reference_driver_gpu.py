@@ -1,5 +1,5 @@
-"""The drop-in claim, executed: the reference's OWN run_pretraining.py (byte-for-byte the file installed from /root/reference by
-baseline/install_ref.py -- checked against the manifest hash) trains over the B200 mirror (shims/ours) with its own flags, writes its
+"""The drop-in claim, executed: the reference's OWN run_pretraining.py (byte for byte, read where it lies in the reference
+checkout) trains over the H100 mirror (shims/ours) with its own flags, writes its
 own checkpoints and resumes from them (run_pretraining.py:388-410,489-515), eagerly and with its own --cuda_graphs.  The same script
 also runs over the reference's own modeling.py + fused_lamb_CUDA kernels (the GPU baseline arm) so that arm is known to work here.
 
@@ -18,7 +18,8 @@ import torch
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref", "BERT")
+sys.path.insert(0, ROOT)
+from oracle.build_ref import REF_BERT as REF  # noqa: E402
 SMALL = dict(attention_probs_dropout_prob=0.1, hidden_act="gelu", hidden_dropout_prob=0.1, hidden_size=256, initializer_range=0.02,
              intermediate_size=1024, max_position_embeddings=128, num_attention_heads=4, num_hidden_layers=2, type_vocab_size=2,
              vocab_size=30522)
@@ -26,7 +27,7 @@ SMALL = dict(attention_probs_dropout_prob=0.1, hidden_act="gelu", hidden_dropout
 
 def _need_ref():
     if not os.path.exists(os.path.join(REF, "run_pretraining.py")):
-        pytest.skip("baseline/_ref/BERT not installed (python baseline/install_ref.py where /root/reference exists)")
+        pytest.skip("no reference checkout (oracle/build_ref.py: REF_BERT; set DLE_REFERENCE_ROOT)")
 
 
 def _run(arm, out, extra, steps, tmp_path, timeout=600):
@@ -59,9 +60,18 @@ def _final(recs, key):
 
 def test_installed_reference_script_is_the_reference_file():
     _need_ref()
-    manifest = json.load(open(os.path.join(REF, "MANIFEST.json")))
-    for rel in ("run_pretraining.py", "modeling.py", "lamb_amp_opt/fused_lamb/fused_lamb.py"):
-        assert hashlib.sha256(open(os.path.join(REF, rel), "rb").read()).hexdigest() == manifest[rel]
+    import importlib.util
+    spec = importlib.util.spec_from_file_location("run_reference_driver", os.path.join(ROOT, "tools", "run_reference_driver.py"))
+    drv = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(drv)
+    saved = list(sys.path)
+    try:
+        script = drv.setup("ours")                    # the script the driver executes over shims/ours
+    finally:
+        sys.path[:] = saved
+    digest = lambda f: hashlib.sha256(open(f, "rb").read()).hexdigest()
+    assert digest(script) == digest(os.path.join(REF, "run_pretraining.py"))
+    assert os.path.dirname(script) != REF             # run alone, so the reference's own modeling.py cannot be picked up
 
 
 @pytest.mark.parametrize("graphs", [False, True])

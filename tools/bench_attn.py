@@ -36,8 +36,8 @@ def main():
         ff, bf = 4.0 * S * S * 64 * B * A, 10.0 * S * S * 64 * B * A
         rows.append(dict(case=name, fwd_us=round(f * 1e3, 1), fwd_tflops=round(ff / f / 1e9, 1), bwd_us=round(b * 1e3, 1), bwd_tflops=round(bf / b / 1e9, 1)))
         print(rows[-1], flush=True)
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump(dict(B=B, S=S, A=A, rows=rows), open("gpurun_out/bench_attn.json", "w"), indent=1)
+    os.makedirs("bench_out", exist_ok=True)
+    json.dump(dict(B=B, S=S, A=A, rows=rows), open("bench_out/bench_attn.json", "w"), indent=1)
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""Encoder-only inference throughput (BASELINE.json configs[4]: BERT-large, S=512, B=256, bf16, eval mode, 1xB200):
+"""Encoder-only inference throughput (BASELINE.json configs[4]: BERT-large, S=512, B=256, bf16, eval mode, 1xH100):
 embeddings + 24 encoder layers + pooler, forward only, CUDA-event timed, eager and as a replayed CUDA graph; full-length batch and a
 variable-length batch (lengths ~ U{S/4..S} rounded up to 64, SURVEY.md 8d) where the attention kernel skips fully padded key tiles.
 FasterTransformer is a README stub in the reference (SURVEY.md 0), so the parity target for this config is the reference BertModel in
@@ -38,4 +38,4 @@ for name, full in (("full-length", True), ("variable-length", False)):
                                 padded_tflops=round(B * fwd / ms / 1e9, 1), real_tokens_per_s=round(tokens / ms * 1e3), token_fill=round(tokens / (B * S), 3)))
         print(out["runs"][-1], flush=True)
 print(json.dumps(out))
-os.makedirs("gpurun_out", exist_ok=True); json.dump(out, open("gpurun_out/bench_infer.json", "w"))
+os.makedirs("bench_out", exist_ok=True); json.dump(out, open("bench_out/bench_infer.json", "w"))

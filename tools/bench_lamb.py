@@ -74,8 +74,8 @@ def main():
                 print("reference", out["reference_fused_lamb_CUDA_fp32"], flush=True)
         del opt, decay, nodecay
         torch.cuda.empty_cache()
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump(dict(hbm_peak_GBps=peak, **out), open("gpurun_out/bench_lamb.json", "w"), indent=1)
+    os.makedirs("bench_out", exist_ok=True)
+    json.dump(dict(hbm_peak_GBps=peak, **out), open("bench_out/bench_lamb.json", "w"), indent=1)
 
 
 if __name__ == "__main__":

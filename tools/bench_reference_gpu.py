@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Time the UNMODIFIED reference training step on the GPU(s) of this box -- the denominator of the north_star's ">= 1.0x the
-reference's own build" -- with exactly the harness bench.py uses for the B200 arm (CUDA events, max over ranks, barrier +
+reference's own build" -- with exactly the harness bench.py uses for the H100 arm (CUDA events, max over ranks, barrier +
 synchronize on both sides, W warm-up steps, K timed steps, resident and end-to-end passes).
 
     python tools/bench_reference_gpu.py --arm reference --batch 32 --steps 8 --warmup 3            # 1 GPU
