@@ -1,17 +1,20 @@
-// Fused multi-head self-attention for sm_90a (head dim 64, S in {128,256,384,512}), on the warp-level tensor-core MMA
-// (mma.sync m16n8k16, bf16 in, fp32 accumulate) with operands fed from XOR-swizzled shared memory by ldmatrix and tiles
-// streamed in by cp.async double buffering.
+// Fused multi-head self-attention for sm_90a (head dim 64, S in {128,256,384,512}) on warpgroup MMA (wgmma.mma_async m64n64k16,
+// bf16 in, fp32 accumulators in registers).  Tiles of 64 rows x 64 bf16 (128-byte rows) are streamed into 1024-byte aligned,
+// 128B-swizzled shared memory by cp.async double buffering and read there by wgmma as K-major or (through the transpose bit)
+// MN-major operands; the P / dS operands go to wgmma from registers.
 //
-// Forward : one CTA per (batch, head, 128-query tile), 8 warps x 16 query rows.  Q stays in registers; K / V come in 64-key
-//           tiles.  S = Q K^T, online softmax in registers, dropout (Philox, regenerated in backward), O += P V with P taken
-//           straight from the S accumulators (as bf16 hi + lo parts).  The [B,A,S,S] score tensor the reference materialises 3x per layer never
-//           exists in HBM.
+// Forward : one CTA per (batch, head, 128-query tile), two warpgroups x 64 query rows.  K / V come in 64-key tiles.
+//           S = Q K^T, online softmax in registers, dropout (Philox, regenerated in backward), O += P V with P taken straight
+//           from the S accumulators (as bf16 hi + lo parts).  The [B,A,S,S] score tensor the reference materialises 3x per layer
+//           never exists in HBM.
 // Backward: two kernels that recompute P from the saved log-sum-exp, so that every output is accumulated on chip by exactly
 //           one CTA -- no atomics on dQ / dK / dV, deterministic:
-//             dK / dV : one CTA per (batch, head, 64-key tile); the warps hold their 16 keys' K and V rows in registers and
-//                       walk the query tiles, computing S^T = K Q^T and dP^T = V dO^T, then dV += P~^T dO, dK += dS^T Q.
-//             dQ      : one CTA per (batch, head, 64-query tile); the warps hold Q and dO rows and walk the key tiles,
-//                       computing S and dP again, then dQ += dS K.
+//             dK / dV : one CTA (one warpgroup) per (batch, head, 64-key tile) walks the query tiles, computing S^T = K Q^T and
+//                       dP^T = V dO^T, then dV += P~^T dO, dK += dS^T Q.
+//             dQ      : one CTA (one warpgroup) per (batch, head, 64-query tile) walks the key tiles, computing S and dP again,
+//                       then dQ += dS K.
+// Dropout: each Philox block (one query row x 32 keys) a CTA needs is computed by one thread, while the tile's score MMAs run,
+//          and handed to the threads that apply it through shared memory.
 //
 // replaces BertSelfAttention.forward, PyTorch/LanguageModeling/BERT/modeling.py:349-376
 // (transpose_for_scores, bmm, /sqrt(d), +mask, softmax, dropout, bmm, transpose+contiguous) and autograd.
@@ -31,8 +34,8 @@ __device__ __forceinline__ float ex2(float x) {
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-// byte offset of 16-byte unit `ch` (8 bf16) of row r in a tile of 128-byte rows, XOR-swizzled by row % 8 so that both the
-// cp.async row writes and the ldmatrix 8-row reads are free of bank conflicts
+// byte offset of 16-byte unit `ch` (8 bf16) of row r in a tile of 128-byte rows, XOR-swizzled by row % 8.  In a 1024-byte aligned
+// tile this is exactly the hardware's 128-byte swizzle, which wgmma descriptors of mode SWIZZLE_128B read.
 __device__ __forceinline__ uint32_t sw(int r, int ch) { return (uint32_t)(r * 128 + ((ch ^ (r & 7)) << 4)); }
 
 struct AttnParams {
@@ -64,45 +67,46 @@ __device__ __forceinline__ void load_tile(uint32_t dst, const bf16* base, long l
         cp_async16(dst + sw(r, ch), base + tok_row(p, b, s0 + r) * ld + col + ch * 8);
     }
 }
-// A fragments (16 rows from r0, all 64 columns = 4 k-steps) of a swizzled tile
-__device__ __forceinline__ void load_a_frags(uint32_t tile, int r0, int lane, uint32_t (&f)[4][4]) {
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) ldsm_x4(tile + sw(r0 + (lane & 15), 2 * kk + (lane >> 4)), f[kk][0], f[kk][1], f[kk][2], f[kk][3]);
+// the cp.async groups up to the newest-but-N are in shared memory and visible to wgmma (async proxy) in every thread of the CTA
+template <int N> __device__ __forceinline__ void tiles_ready() {
+    cp_async_wait<N>();
+    fence_proxy_async_smem();
+    __syncthreads();
 }
-// acc[16 x 64] = A[16 x 64] * T^T where tile T holds 64 rows (the n dimension) of 64 columns (the k dimension)
-__device__ __forceinline__ void mma_abt(float (&acc)[8][4], const uint32_t (&a)[4][4], uint32_t tile, int lane) {
+// acc[64 x 64] = A * T^T, A = 64 rows of 64 columns at `a` (K-major), T = 64 rows (the n dimension) of 64 columns at `t` (K-major).
+// Issued only: the caller fences, commits and waits.
+__device__ __forceinline__ void wg_abt(float (&acc)[8][4], uint32_t a, uint32_t t) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.f;
+    for (int kk = 0; kk < 4; ++kk)
+        wgmma_m64n64k16<0, 0>(acc, make_wgmma_desc_sw128(a + kk * 32, 16, 1024), make_wgmma_desc_sw128(t + kk * 32, 16, 1024), kk > 0 ? 1u : 0u);
+}
+// acc[64 x 64] += A * T, A = packed bf16 accumulator pairs (pr[j][0]: row r, pr[j][1]: row r + 8 of column block j) and tile T
+// holding 64 rows (the k dimension) of 64 columns (the n dimension), read MN-major.  Issued only.
+__device__ __forceinline__ void wg_pt(float (&acc)[8][4], const uint32_t (&pr)[8][2], uint32_t t) {
 #pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
+    for (int kk = 0; kk < 4; ++kk)
+        wgmma_m64n64k16_rs<1>(acc, pr[2 * kk][0], pr[2 * kk][1], pr[2 * kk + 1][0], pr[2 * kk + 1][1],
+                              make_wgmma_desc_sw128(t + kk * 16 * 128, TILE64_BYTES, 1024));
+}
+// Row-major dropout (forward, dQ): a warp owns 16 query rows; per 64-key tile it needs the Philox blocks of its 16 rows x 2 key
+// groups.  Lane l computes the block of row (first + l % 16), group l / 16 into slot l of the warp's 512-byte area; after __syncwarp
+// the four lanes of a quad read the blocks of their rows r and r + 8 (broadcast).  drop_row = (bh*S + first row of the warp)*S.
+__device__ __forceinline__ void warp_drop_blocks(uint4* slots, unsigned long long seed, uint32_t stream, unsigned long long drop_row,
+                                                 int S, int key0, int lane) {
+    slots[lane] = attn_dropout_block(seed, stream, (drop_row + (unsigned long long)(lane & 15) * S + key0 + (lane >> 4) * 32) >> 5);
+}
+// keep words of the packed pairs of rows r (k[j][0]) and r + 8 (k[j][1]) in column block j, from the warp's slots
+__device__ __forceinline__ void warp_drop_words(const uint4* slots, uint32_t k2, int lane, uint32_t (&k)[8][2]) {
+    const int r = lane >> 2;
 #pragma unroll
-        for (int np = 0; np < 4; ++np) {
-            uint32_t b0, b1, b2, b3;
-            ldsm_x4(tile + sw(16 * np + (lane & 7) + ((lane >> 4) << 3), 2 * kk + ((lane >> 3) & 1)), b0, b1, b2, b3);
-            mma_bf16_16816(acc[2 * np], a[kk], b0, b1);
-            mma_bf16_16816(acc[2 * np + 1], a[kk], b2, b3);
+    for (int g = 0; g < 2; ++g) {
+        const uint4 ra = slots[g * 16 + r], rb = slots[g * 16 + r + 8];
+#pragma unroll
+        for (int w = 0; w < 4; ++w) {                             // column block j = 4g + w holds pair word 4w + lane % 4
+            k[4 * g + w][0] = attn_dropout_word(ra, 4 * w + (lane & 3), k2);
+            k[4 * g + w][1] = attn_dropout_word(rb, 4 * w + (lane & 3), k2);
         }
     }
-}
-// acc[16 x 64] += A[16 x 64] * T where A arrives as packed bf16 accumulator pairs (pr[j][0]: row r, pr[j][1]: row r + 8 of
-// column tile j) and tile T holds 64 rows (the k dimension) of 64 columns (the n dimension)
-__device__ __forceinline__ void mma_pt(float (&acc)[8][4], const uint32_t (&pr)[8][2], uint32_t tile, int lane) {
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-        const uint32_t a[4] = {pr[2 * kk][0], pr[2 * kk][1], pr[2 * kk + 1][0], pr[2 * kk + 1][1]};
-#pragma unroll
-        for (int np = 0; np < 4; ++np) {
-            uint32_t b0, b1, b2, b3;
-            ldsm_x4_trans(tile + sw(16 * kk + (lane & 7) + (((lane >> 3) & 1) << 3), 2 * np + (lane >> 4)), b0, b1, b2, b3);
-            mma_bf16_16816(acc[2 * np], a, b0, b1);
-            mma_bf16_16816(acc[2 * np + 1], a, b2, b3);
-        }
-    }
-}
-// 16-bit keep mask of one element: 0xFFFF (kept) or 0
-__device__ __forceinline__ uint32_t keep_half(const uint4& r, int key, uint32_t k2) {
-    const uint32_t w = attn_dropout_word(r, (key & 31) >> 1, k2);
-    return (key & 1) ? (w >> 16) : (w & 0xFFFFu);
 }
 // bf16 rows [r0, r0+16) x 64 columns of a fragment accumulator -> dqkv column block `col`; column sums of the stored values -> dbias
 __device__ __forceinline__ void store_rows_bf16(const AttnParams& p, const float (&acc)[8][4], float mul, int b, int s_row0, int col, int lane) {
@@ -123,21 +127,28 @@ __device__ __forceinline__ void store_rows_bf16(const AttnParams& p, const float
         }
     }
 }
+// dynamic shared memory rounded up to the 1024-byte alignment of the swizzled tiles
+__device__ __forceinline__ uint8_t* smem_1k(uint8_t* smem) {
+    return smem + (((smem_u32(smem) + 1023u) & ~1023u) - smem_u32(smem));
+}
 
 // =================================================================================================
 // forward
 // =================================================================================================
 constexpr int FWD_WARPS = 8, FWD_THREADS = FWD_WARPS * 32, FWD_TQ = FWD_WARPS * 16;
-constexpr int FWD_SMEM_BYTES = 2 * TILE64_BYTES /*Q*/ + 4 * TILE64_BYTES /*K, V x 2*/ + 512 * 4 /*mask*/;
+constexpr int FWD_SMEM_BYTES = 1024 /*alignment*/ + 2 * TILE64_BYTES /*Q*/ + 4 * TILE64_BYTES /*K, V x 2*/ + 512 * 4 /*mask*/
+                             + FWD_WARPS * 512 /*Philox blocks*/;
 
-__global__ void __launch_bounds__(FWD_THREADS)
+__global__ void __launch_bounds__(FWD_THREADS, 2)
 attn_fwd_kernel(const AttnParams p) {
-    extern __shared__ __align__(128) uint8_t smem[];
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_1k(smem_raw);
     const int S = p.S, nkt = S / KT;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
     const uint32_t sQ = smem_u32(smem), sK = sQ + 2 * TILE64_BYTES, sV = sK + 2 * TILE64_BYTES;
     float* sMask = reinterpret_cast<float*>(smem + 6 * TILE64_BYTES);      // additive mask of the key row, times log2(e)
+    uint4* sRng = reinterpret_cast<uint4*>(smem + 6 * TILE64_BYTES + 512 * 4) + warp * 32;
     const long long ld = 3LL * p.H;
 
     load_tile<FWD_TQ, FWD_THREADS>(sQ, p.qkv, ld, h * HD, p, b, qt * FWD_TQ);
@@ -148,10 +159,9 @@ attn_fwd_kernel(const AttnParams p) {
 
     const int r = lane >> 2, c = 2 * (lane & 3);
     const int q0 = qt * FWD_TQ + warp * 16 + r;                  // query rows q0 and q0 + 8 of this thread
+    const uint32_t sQw = sQ + (warp >> 2) * TILE64_BYTES;        // the 64 query rows of this warpgroup
     const unsigned long long seed = effective_seed(p.seed, p.seed_dev);
-    const unsigned long long drop_row0 = ((unsigned long long)(b * p.A + h) * S + q0) * (unsigned long long)S;
-    const unsigned long long drop_row1 = drop_row0 + 8ull * S;
-    uint32_t qf[4][4];
+    const unsigned long long drop_row = ((unsigned long long)(b * p.A + h) * S + qt * FWD_TQ + warp * 16) * (unsigned long long)S;
     float o[8][4];
 #pragma unroll
     for (int j = 0; j < 8; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
@@ -164,11 +174,15 @@ attn_fwd_kernel(const AttnParams p) {
             load_tile<KT, FWD_THREADS>(sV + (buf ^ 1) * TILE64_BYTES, p.qkv, ld, 2 * p.H + h * HD, p, b, (kt + 1) * KT);
         }
         cp_async_commit();
-        cp_async_wait<1>();
-        __syncthreads();
-        if (kt == 0) load_a_frags(sQ, warp * 16, lane, qf);
+        tiles_ready<1>();
         float s[8][4];
-        mma_abt(s, qf, sK + buf * TILE64_BYTES, lane);
+        wgmma_fence();
+        wg_abt(s, sQw, sK + buf * TILE64_BYTES);                 // S = Q K^T, in flight during the Philox blocks
+        wgmma_commit();
+        if (p.drop_on != 0u) warp_drop_blocks(sRng, seed, p.drop_stream, drop_row, S, kt * KT, lane);
+        __syncwarp();
+        wgmma_wait<0>();
+        fence_regs(s);
         // ---- scale + mask (log2 domain), row maxima over the quad
         float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
@@ -201,22 +215,18 @@ attn_fwd_kernel(const AttnParams p) {
             pl[j][0] = pack_bf16(e0 - h0.x, e1 - h0.y); pl[j][1] = pack_bf16(e2 - h1.x, e3 - h1.y);
         }
         if (p.drop_on != 0u) {
+            uint32_t km[8][2];
+            warp_drop_words(sRng, p.drop_k2, lane, km);
 #pragma unroll
-            for (int g = 0; g < 2; ++g) {                                 // the two 32-key RNG groups of the tile
-                const int key0 = kt * KT + g * 32;
-                const uint4 ra = attn_dropout_block(seed, p.drop_stream, (drop_row0 + key0) >> 5);
-                const uint4 rb = attn_dropout_block(seed, p.drop_stream, (drop_row1 + key0) >> 5);
-#pragma unroll
-                for (int w = 0; w < 4; ++w) {                             // column tile j = 4g + w holds pair word 4w + lane % 4
-                    const uint32_t ka = attn_dropout_word(ra, 4 * w + (lane & 3), p.drop_k2);
-                    const uint32_t kb = attn_dropout_word(rb, 4 * w + (lane & 3), p.drop_k2);
-                    pr[4 * g + w][0] &= ka; pl[4 * g + w][0] &= ka;
-                    pr[4 * g + w][1] &= kb; pl[4 * g + w][1] &= kb;
-                }
-            }
+            for (int j = 0; j < 8; ++j) { pr[j][0] &= km[j][0]; pl[j][0] &= km[j][0]; pr[j][1] &= km[j][1]; pl[j][1] &= km[j][1]; }
         }
-        mma_pt(o, pr, sV + buf * TILE64_BYTES, lane);
-        mma_pt(o, pl, sV + buf * TILE64_BYTES, lane);
+        fence_regs(o);
+        wgmma_fence();
+        wg_pt(o, pr, sV + buf * TILE64_BYTES);
+        wg_pt(o, pl, sV + buf * TILE64_BYTES);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(o); fence_regs(pr); fence_regs(pl);
         __syncthreads();                                                  // buffer `buf` is refilled at the next iteration
     }
     // ---- epilogue: O * (1/(1-p)) / l -> ctx, lse
@@ -240,9 +250,13 @@ attn_fwd_kernel(const AttnParams p) {
 // =================================================================================================
 // backward
 // =================================================================================================
-constexpr int BWD_WARPS = 4, BWD_THREADS = BWD_WARPS * 32;
-// K, V (or Q, dO) of the CTA's own tile + a double-buffered pair of streamed tiles + per-row statistics / mask
-constexpr int BWD_SMEM_BYTES = 2 * TILE64_BYTES + 4 * TILE64_BYTES + 4 * 512 * 4;
+constexpr int BWD_THREADS = 128;       // one warpgroup
+// dK/dV keep words of one query tile: word i (0..15) of the Philox block of (query ql, key group g) at [(g*16 + i) * KEEP_LD + ql];
+// the padding makes both the producer's row writes and the consumers' (ql, ql+1) pair reads free of bank conflicts
+constexpr int KEEP_LD = 72;
+constexpr int KEEP_BYTES = 32 * KEEP_LD * 4;
+constexpr int BWD_DKV_SMEM_BYTES = 1024 + 6 * TILE64_BYTES + 2 * 512 * 4 /*-lse, -delta*/ + 2 * KEEP_BYTES;
+constexpr int BWD_DQ_SMEM_BYTES = 1024 + 6 * TILE64_BYTES + 512 * 4 /*mask*/ + 4 * 512 /*Philox blocks*/;
 
 // delta[b,h,s] = sum_d dO[t, h*64+d] * O[t, h*64+d].  Eight lanes share one (token, head) row: consecutive lanes read consecutive
 // 16-byte units, so a warp instruction covers 4 whole 128-byte lines.
@@ -272,6 +286,16 @@ __global__ void attn_delta_kernel(const bf16* __restrict__ dctx, const bf16* __r
     }
 }
 
+// the 64 queries x 2 key groups of query tile qt against key tile kt: thread t computes the Philox block of (query t % 64, group
+// t / 64) and all 16 of its pair words
+__device__ __forceinline__ void dkv_keep_words(uint32_t* keep, const AttnParams& p, unsigned long long seed, long long bh, int kt, int qt) {
+    const int ql = threadIdx.x & 63, g = threadIdx.x >> 6;
+    const unsigned long long row = (unsigned long long)(bh * p.S + qt * KT + ql) * (unsigned long long)p.S;
+    const uint4 blk = attn_dropout_block(seed, p.drop_stream, (row + kt * KT + g * 32) >> 5);
+#pragma unroll
+    for (int i = 0; i < 16; ++i) keep[(g * 16 + i) * KEEP_LD + ql] = attn_dropout_word(blk, i, p.drop_k2);
+}
+
 // dK, dV of one 64-key tile.  Thread layout of the transposed score tile: key rows kr, kr + 8 (kr = tile + warp*16 + lane/4),
 // query columns 8j + 2(lane%4) + {0,1} of the current query tile.
 //   P   = exp2(S * scale*log2e + mask*log2e - lse*log2e)          (bf16, as in forward)
@@ -280,13 +304,15 @@ __global__ void attn_delta_kernel(const bf16* __restrict__ dctx, const bf16* __r
 //   dV += P~^T dO (times 1/(1-p) at the end),  dK += dS^T Q
 __global__ void __launch_bounds__(BWD_THREADS)
 attn_bwd_dkv_kernel(const AttnParams p) {
-    extern __shared__ __align__(128) uint8_t smem[];
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_1k(smem_raw);
     const int S = p.S, nqt = S / KT;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int kt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
     const uint32_t sK = smem_u32(smem), sV = sK + TILE64_BYTES, sQ = sV + TILE64_BYTES, sdO = sQ + 2 * TILE64_BYTES;
     float* sLse = reinterpret_cast<float*>(smem + 6 * TILE64_BYTES);          // [S] -lse*log2e
     float* sNd = sLse + 512;                                                   // [S] -delta*scale
+    uint32_t* sKeep = reinterpret_cast<uint32_t*>(sNd + 512);                  // 2 x [32 x KEEP_LD] keep words
     const long long ld = 3LL * p.H;
     const long long bh = (long long)b * p.A + h;
 
@@ -296,14 +322,17 @@ attn_bwd_dkv_kernel(const AttnParams p) {
     load_tile<KT, BWD_THREADS>(sdO, p.dctx, p.H, h * HD, p, b, 0);
     cp_async_commit();
     for (int i = threadIdx.x; i < S; i += BWD_THREADS) { sLse[i] = -p.lse[bh * S + i] * LOG2E; sNd[i] = -p.delta[bh * S + i] * p.scale; }
+    const unsigned long long seed = effective_seed(p.seed, p.seed_dev);
+    if (p.drop_on != 0u) dkv_keep_words(sKeep, p, seed, bh, kt, 0);
 
     const int r = lane >> 2, c = 2 * (lane & 3);
     const int kr = kt * KT + warp * 16 + r;                      // key rows kr and kr + 8 of this thread
     const float mk0 = p.mask ? p.mask[(long long)b * S + kr] * LOG2E : 0.f;
     const float mk1 = p.mask ? p.mask[(long long)b * S + kr + 8] * LOG2E : 0.f;
-    const unsigned long long seed = effective_seed(p.seed, p.seed_dev);
+    // keys kr and kr + 8 are halves (r & 1) of pair words i and i + 4 of key group warp / 2, for every query
+    const int keep_row = (warp >> 1) * 16 + (warp & 1) * 8 + (r >> 1);
+    const uint32_t half_sel = (r & 1) ? 0x7632u : 0x5410u;
     const float c1 = p.drop_scale * p.scale;
-    uint32_t kf[4][4], vf[4][4];
     float dk[8][4], dv[8][4];
 #pragma unroll
     for (int j = 0; j < 8; ++j) { dk[j][0] = dk[j][1] = dk[j][2] = dk[j][3] = 0.f; dv[j][0] = dv[j][1] = dv[j][2] = dv[j][3] = 0.f; }
@@ -315,13 +344,18 @@ attn_bwd_dkv_kernel(const AttnParams p) {
             load_tile<KT, BWD_THREADS>(sdO + (buf ^ 1) * TILE64_BYTES, p.dctx, p.H, h * HD, p, b, (qt + 1) * KT);
         }
         cp_async_commit();
-        cp_async_wait<1>();
-        __syncthreads();
-        if (qt == 0) { load_a_frags(sK, warp * 16, lane, kf); load_a_frags(sV, warp * 16, lane, vf); }
+        tiles_ready<1>();                                        // also publishes the keep words of this query tile
         const uint32_t tQ = sQ + buf * TILE64_BYTES, tdO = sdO + buf * TILE64_BYTES;
         float st[8][4], dpt[8][4];
-        mma_abt(st, kf, tQ, lane);                               // S^T  = K Q^T
-        mma_abt(dpt, vf, tdO, lane);                             // dP^T = V dO^T
+        wgmma_fence();
+        wg_abt(st, sK, tQ);                                      // S^T  = K Q^T
+        wg_abt(dpt, sV, tdO);                                    // dP^T = V dO^T
+        wgmma_commit();
+        // while the MMAs run: the keep words of the next query tile (read after the next iteration's barrier)
+        if (p.drop_on != 0u && qt + 1 < nqt) dkv_keep_words(sKeep + ((qt + 1) & 1) * (32 * KEEP_LD), p, seed, bh, kt, qt + 1);
+        wgmma_wait<0>();
+        fence_regs(st); fence_regs(dpt);
+        const uint32_t* keep = sKeep + buf * (32 * KEEP_LD) + keep_row * KEEP_LD;
         uint32_t pm[8][2], ds[8][2];
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -331,20 +365,24 @@ attn_bwd_dkv_kernel(const AttnParams p) {
             const uint32_t p0 = pack_bf16(ex2(fmaf(st[j][0], p.scale_log2, mk0) + nl.x), ex2(fmaf(st[j][1], p.scale_log2, mk0) + nl.y));
             const uint32_t p1 = pack_bf16(ex2(fmaf(st[j][2], p.scale_log2, mk1) + nl.x), ex2(fmaf(st[j][3], p.scale_log2, mk1) + nl.y));
             uint32_t k0 = 0xFFFFFFFFu, k1 = 0xFFFFFFFFu;
-            if (p.drop_on != 0u) {                               // keys kr and kr + 8 share the 32-element group of each query
-                const unsigned long long row = (unsigned long long)(bh * S + q) * (unsigned long long)S;
-                const uint4 ra = attn_dropout_block(seed, p.drop_stream, (row + kr) >> 5);
-                const uint4 rb = attn_dropout_block(seed, p.drop_stream, (row + S + kr) >> 5);
-                k0 = keep_half(ra, kr, p.drop_k2) | (keep_half(rb, kr, p.drop_k2) << 16);
-                k1 = keep_half(ra, kr + 8, p.drop_k2) | (keep_half(rb, kr + 8, p.drop_k2) << 16);
+            if (p.drop_on != 0u) {
+                const uint2 wa = *reinterpret_cast<const uint2*>(keep + j * 8 + c);                 // word i of queries q, q + 1
+                const uint2 wb = *reinterpret_cast<const uint2*>(keep + 4 * KEEP_LD + j * 8 + c);   // word i + 4
+                k0 = prmt(wa.x, wa.y, half_sel);
+                k1 = prmt(wb.x, wb.y, half_sel);
             }
             pm[j][0] = p0 & k0; pm[j][1] = p1 & k1;
             const float2 f0 = unpack_bf16(p0), f1 = unpack_bf16(p1), g0 = unpack_bf16(pm[j][0]), g1 = unpack_bf16(pm[j][1]);
             ds[j][0] = pack_bf16(fmaf(g0.x * dpt[j][0], c1, f0.x * nd.x), fmaf(g0.y * dpt[j][1], c1, f0.y * nd.y));
             ds[j][1] = pack_bf16(fmaf(g1.x * dpt[j][2], c1, f1.x * nd.x), fmaf(g1.y * dpt[j][3], c1, f1.y * nd.y));
         }
-        mma_pt(dv, pm, tdO, lane);                               // dV += P~^T dO
-        mma_pt(dk, ds, tQ, lane);                                // dK += dS^T Q
+        fence_regs(dv); fence_regs(dk);
+        wgmma_fence();
+        wg_pt(dv, pm, tdO);                                      // dV += P~^T dO
+        wg_pt(dk, ds, tQ);                                       // dK += dS^T Q
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(dv); fence_regs(dk); fence_regs(pm); fence_regs(ds);
         __syncthreads();
     }
     const int s_row0 = kt * KT + warp * 16;
@@ -355,12 +393,14 @@ attn_bwd_dkv_kernel(const AttnParams p) {
 // dQ of one 64-query tile: rows q, q + 8 (q = tile + warp*16 + lane/4), key columns of the current key tile.  dQ += dS K.
 __global__ void __launch_bounds__(BWD_THREADS)
 attn_bwd_dq_kernel(const AttnParams p) {
-    extern __shared__ __align__(128) uint8_t smem[];
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_1k(smem_raw);
     const int S = p.S, nkt = S / KT;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
     const uint32_t sQ = smem_u32(smem), sdO = sQ + TILE64_BYTES, sK = sdO + TILE64_BYTES, sV = sK + 2 * TILE64_BYTES;
     float* sMask = reinterpret_cast<float*>(smem + 6 * TILE64_BYTES);
+    uint4* sRng = reinterpret_cast<uint4*>(smem + 6 * TILE64_BYTES + 512 * 4) + warp * 32;
     const long long ld = 3LL * p.H;
     const long long bh = (long long)b * p.A + h;
 
@@ -376,10 +416,8 @@ attn_bwd_dq_kernel(const AttnParams p) {
     const float nl0 = -p.lse[bh * S + q0] * LOG2E, nl1 = -p.lse[bh * S + q0 + 8] * LOG2E;
     const float nd0 = -p.delta[bh * S + q0] * p.scale, nd1 = -p.delta[bh * S + q0 + 8] * p.scale;
     const unsigned long long seed = effective_seed(p.seed, p.seed_dev);
-    const unsigned long long drop_row0 = (unsigned long long)(bh * S + q0) * (unsigned long long)S;
-    const unsigned long long drop_row1 = drop_row0 + 8ull * S;
+    const unsigned long long drop_row = (unsigned long long)(bh * S + qt * KT + warp * 16) * (unsigned long long)S;
     const float c1 = p.drop_scale * p.scale;
-    uint32_t qf[4][4], of[4][4];
     float dq[8][4];
 #pragma unroll
     for (int j = 0; j < 8; ++j) dq[j][0] = dq[j][1] = dq[j][2] = dq[j][3] = 0.f;
@@ -391,29 +429,21 @@ attn_bwd_dq_kernel(const AttnParams p) {
             load_tile<KT, BWD_THREADS>(sV + (buf ^ 1) * TILE64_BYTES, p.qkv, ld, 2 * p.H + h * HD, p, b, (kt + 1) * KT);
         }
         cp_async_commit();
-        cp_async_wait<1>();
-        __syncthreads();
-        if (kt == 0) { load_a_frags(sQ, warp * 16, lane, qf); load_a_frags(sdO, warp * 16, lane, of); }
+        tiles_ready<1>();
         const uint32_t tK = sK + buf * TILE64_BYTES, tV = sV + buf * TILE64_BYTES;
         float s[8][4], dp[8][4];
-        mma_abt(s, qf, tK, lane);                                // S  = Q K^T
-        mma_abt(dp, of, tV, lane);                               // dP = dO V^T
+        wgmma_fence();
+        wg_abt(s, sQ, tK);                                       // S  = Q K^T
+        wg_abt(dp, sdO, tV);                                     // dP = dO V^T
+        wgmma_commit();
+        if (p.drop_on != 0u) warp_drop_blocks(sRng, seed, p.drop_stream, drop_row, S, kt * KT, lane);
+        __syncwarp();
         uint32_t km[8][2];
 #pragma unroll
         for (int j = 0; j < 8; ++j) km[j][0] = km[j][1] = 0xFFFFFFFFu;
-        if (p.drop_on != 0u) {
-#pragma unroll
-            for (int g = 0; g < 2; ++g) {
-                const int key0 = kt * KT + g * 32;
-                const uint4 ra = attn_dropout_block(seed, p.drop_stream, (drop_row0 + key0) >> 5);
-                const uint4 rb = attn_dropout_block(seed, p.drop_stream, (drop_row1 + key0) >> 5);
-#pragma unroll
-                for (int w = 0; w < 4; ++w) {
-                    km[4 * g + w][0] = attn_dropout_word(ra, 4 * w + (lane & 3), p.drop_k2);
-                    km[4 * g + w][1] = attn_dropout_word(rb, 4 * w + (lane & 3), p.drop_k2);
-                }
-            }
-        }
+        if (p.drop_on != 0u) warp_drop_words(sRng, p.drop_k2, lane, km);
+        wgmma_wait<0>();
+        fence_regs(s); fence_regs(dp);
         uint32_t ds[8][2];
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -424,7 +454,12 @@ attn_bwd_dq_kernel(const AttnParams p) {
             ds[j][0] = pack_bf16(fmaf(g0.x * dp[j][0], c1, f0.x * nd0), fmaf(g0.y * dp[j][1], c1, f0.y * nd0));
             ds[j][1] = pack_bf16(fmaf(g1.x * dp[j][2], c1, f1.x * nd1), fmaf(g1.y * dp[j][3], c1, f1.y * nd1));
         }
-        mma_pt(dq, ds, tK, lane);                                // dQ += dS K
+        fence_regs(dq);
+        wgmma_fence();
+        wg_pt(dq, ds, tK);                                       // dQ += dS K
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(dq); fence_regs(ds);
         __syncthreads();
     }
     store_rows_bf16(p, dq, 1.0f, b, qt * KT + warp * 16, h * HD, lane);
@@ -499,13 +534,13 @@ extern "C" int dle_attn_bwd(const void* qkv, const float* mask, const void* ctx,
     attn_common(p, qkv, mask, B, S, A, seq_first, dropout_p, seed, seed_dev, dropout_stream);
     p.dctx = reinterpret_cast<const bf16*>(dctx); p.lse = lse; p.delta = delta_ws; p.dbias = dbias_qkv; p.dqkv = reinterpret_cast<bf16*>(dqkv);
     static SmemAttrCache attr_kv, attr_q;
-    int rc = ensure_smem_attr(attn_bwd_dkv_kernel, attr_kv, BWD_SMEM_BYTES);
+    int rc = ensure_smem_attr(attn_bwd_dkv_kernel, attr_kv, BWD_DKV_SMEM_BYTES);
     if (rc != DLE_OK) return rc;
-    rc = ensure_smem_attr(attn_bwd_dq_kernel, attr_q, BWD_SMEM_BYTES);
+    rc = ensure_smem_attr(attn_bwd_dq_kernel, attr_q, BWD_DQ_SMEM_BYTES);
     if (rc != DLE_OK) return rc;
-    attn_bwd_dkv_kernel<<<dim3(S / KT, A, B), BWD_THREADS, BWD_SMEM_BYTES, st>>>(p);
+    attn_bwd_dkv_kernel<<<dim3(S / KT, A, B), BWD_THREADS, BWD_DKV_SMEM_BYTES, st>>>(p);
     DLE_LAUNCH_CHECK();
-    attn_bwd_dq_kernel<<<dim3(S / KT, A, B), BWD_THREADS, BWD_SMEM_BYTES, st>>>(p);
+    attn_bwd_dq_kernel<<<dim3(S / KT, A, B), BWD_THREADS, BWD_DQ_SMEM_BYTES, st>>>(p);
     DLE_LAUNCH_CHECK();
     return DLE_OK;
 }
