@@ -42,19 +42,26 @@ __device__ __forceinline__ float warp_max(float v) {
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
 }
+// One halving step of warp_column_sums32.  HALF is a template parameter so that every index into v is a compile-time constant:
+// nvcc does not fully unroll a loop over `half >>= 1`, and one run-time index into v puts the whole array, and every epilogue
+// row that flows into it, on the stack.
+template <int HALF> __device__ __forceinline__ void column_sums_halve(float (&v)[32], int lane) {
+    const bool hi = (lane & HALF) != 0;
+#pragma unroll
+    for (int i = 0; i < HALF; ++i) {
+        const float send = hi ? v[i] : v[i + HALF];
+        const float keep = hi ? v[i + HALF] : v[i];
+        v[i] = keep + __shfl_xor_sync(0xffffffffu, send, HALF);
+    }
+}
 // Column sums of a 32x32 tile held one ROW per lane (v[c] = element (lane, c)): recursive halving, 31 shuffles + 31 adds.
 // On return lane l holds the sum over the 32 rows of COLUMN l.
 __device__ __forceinline__ float warp_column_sums32(float (&v)[32], int lane) {
-#pragma unroll
-    for (int half = 16; half >= 1; half >>= 1) {
-        const bool hi = (lane & half) != 0;
-#pragma unroll
-        for (int i = 0; i < half; ++i) {
-            const float send = hi ? v[i] : v[i + half];
-            const float keep = hi ? v[i + half] : v[i];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, half);
-        }
-    }
+    column_sums_halve<16>(v, lane);
+    column_sums_halve<8>(v, lane);
+    column_sums_halve<4>(v, lane);
+    column_sums_halve<2>(v, lane);
+    column_sums_halve<1>(v, lane);
     return v[0];
 }
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
