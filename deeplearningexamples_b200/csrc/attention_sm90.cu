@@ -7,6 +7,8 @@
 //           S = Q K^T, online softmax in registers, dropout (Philox, regenerated in backward), O += P V with P taken straight
 //           from the S accumulators (as bf16 hi + lo parts).  The [B,A,S,S] score tensor the reference materialises 3x per layer
 //           never exists in HBM.
+// Varlen  : the forward for inference over packed sequences (cu_seqlens, any length up to 512): no mask, no dropout, no lse; each
+//           sequence visits only its own key tiles.
 // Backward: two kernels that recompute P from the saved log-sum-exp, so that every output is accumulated on chip by exactly
 //           one CTA -- no atomics on dQ / dK / dV, deterministic:
 //             dK / dV : one CTA (one warpgroup) per (batch, head, 64-key tile) walks the query tiles, computing S^T = K Q^T and
@@ -244,6 +246,132 @@ attn_fwd_kernel(const AttnParams p) {
         float* lse = p.lse_out + ((long long)b * p.A + h) * S;
         lse[q0] = (m0 + log2f(l0)) * LN2;
         lse[q0 + 8] = (m1 + log2f(l1)) * LN2;
+    }
+}
+
+// =================================================================================================
+// variable-length forward (inference): packed tokens, no mask, no dropout, no lse
+// =================================================================================================
+struct VarlenParams {
+    const bf16* qkv;           // [T, 3H], sequence b at rows cu_seqlens[b] .. cu_seqlens[b+1]
+    const int* cu_seqlens;     // [B+1]
+    bf16* ctx;                 // [T, H]
+    int max_seqlen, H;
+    float scale_log2;
+};
+constexpr int FWD_VARLEN_SMEM_BYTES = 1024 /*alignment*/ + 2 * TILE64_BYTES /*Q*/ + 4 * TILE64_BYTES /*K, V x 2*/;
+
+// rows [s0, s0 + ROWS) of a sequence of `len` rows starting at token row `row0`, 64-column block `col` -> swizzled smem tile.  Rows at
+// or past len are zero-filled; their source address is clamped to row0 (len >= 1 here), so no other sequence's row is read.
+template <int ROWS, int NT>
+__device__ __forceinline__ void load_tile_varlen(uint32_t dst, const bf16* base, long long ld, int col, long long row0, int len, int s0) {
+#pragma unroll
+    for (int i = 0; i < ROWS * 8 / NT; ++i) {
+        const int idx = threadIdx.x + i * NT, r = idx >> 3, ch = idx & 7;
+        const bool in = s0 + r < len;
+        cp_async16_zfill(dst + sw(r, ch), base + (row0 + (in ? s0 + r : 0)) * ld + col + ch * 8, in ? 16u : 0u);
+    }
+}
+
+// The tile body is attn_fwd_kernel's with the mask and dropout taken out.  A valid score goes through the same operations as there
+// (fmaf with a zero addend; the padded kernel's extra terms for masked keys are exact zeros), so a row of a sequence gets the bits the
+// padded kernel gives it under a -10000 mask of its padding.  Launched with FWD_THREADS threads; the register cap (instead of
+// __launch_bounds__(FWD_THREADS, 2), which lets ptxas take 127) keeps it at attn_fwd_kernel's budget with no spills: 2 CTAs per SM.
+__global__ void __maxnreg__(120)
+attn_fwd_varlen_kernel(const VarlenParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_1k(smem_raw);
+    const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+    const long long row0 = p.cu_seqlens[b];
+    const int len = max(0, min(p.cu_seqlens[b + 1] - (int)row0, p.max_seqlen));
+    if (qt * FWD_TQ >= len) return;                              // CTA-uniform
+    const int nkt = (len + KT - 1) / KT;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t sQ = smem_u32(smem), sK = sQ + 2 * TILE64_BYTES, sV = sK + 2 * TILE64_BYTES;
+    const long long ld = 3LL * p.H;
+
+    load_tile_varlen<FWD_TQ, FWD_THREADS>(sQ, p.qkv, ld, h * HD, row0, len, qt * FWD_TQ);
+    load_tile_varlen<KT, FWD_THREADS>(sK, p.qkv, ld, p.H + h * HD, row0, len, 0);
+    load_tile_varlen<KT, FWD_THREADS>(sV, p.qkv, ld, 2 * p.H + h * HD, row0, len, 0);
+    cp_async_commit();
+
+    const int r = lane >> 2, c = 2 * (lane & 3);
+    const int q0 = qt * FWD_TQ + warp * 16 + r;                  // query rows q0 and q0 + 8 of this thread
+    const uint32_t sQw = sQ + (warp >> 2) * TILE64_BYTES;
+    float o[8][4];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o[j][0] = o[j][1] = o[j][2] = o[j][3] = 0.f;
+    float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;
+
+    for (int kt = 0; kt < nkt; ++kt) {
+        const int buf = kt & 1;
+        if (kt + 1 < nkt) {
+            load_tile_varlen<KT, FWD_THREADS>(sK + (buf ^ 1) * TILE64_BYTES, p.qkv, ld, p.H + h * HD, row0, len, (kt + 1) * KT);
+            load_tile_varlen<KT, FWD_THREADS>(sV + (buf ^ 1) * TILE64_BYTES, p.qkv, ld, 2 * p.H + h * HD, row0, len, (kt + 1) * KT);
+        }
+        cp_async_commit();
+        tiles_ready<1>();
+        float s[8][4];
+        wgmma_fence();
+        wg_abt(s, sQw, sK + buf * TILE64_BYTES);                 // S = Q K^T
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(s);
+        // ---- scale (log2 domain); keys at or past len (last tile only) -> -inf; row maxima over the quad
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            s[j][0] = fmaf(s[j][0], p.scale_log2, 0.f); s[j][1] = fmaf(s[j][1], p.scale_log2, 0.f);
+            s[j][2] = fmaf(s[j][2], p.scale_log2, 0.f); s[j][3] = fmaf(s[j][3], p.scale_log2, 0.f);
+        }
+        if ((kt + 1) * KT > len) {
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int key = kt * KT + j * 8 + c;
+                if (key >= len) { s[j][0] = -INFINITY; s[j][2] = -INFINITY; }
+                if (key + 1 >= len) { s[j][1] = -INFINITY; s[j][3] = -INFINITY; }
+            }
+        }
+        float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { mx0 = fmaxf(mx0, fmaxf(s[j][0], s[j][1])); mx1 = fmaxf(mx1, fmaxf(s[j][2], s[j][3])); }
+#pragma unroll
+        for (int off = 1; off < 4; off <<= 1) {
+            mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, off)); mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, off));
+        }
+        const float mn0 = fmaxf(m0, mx0), mn1 = fmaxf(m1, mx1);    // finite: every tile holds key kt*64 < len
+        const float al0 = ex2(m0 - mn0), al1 = ex2(m1 - mn1);
+        m0 = mn0; m1 = mn1;
+        l0 *= al0; l1 *= al1;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) { o[j][0] *= al0; o[j][1] *= al0; o[j][2] *= al1; o[j][3] *= al1; }
+        uint32_t pr[8][2], pl[8][2];                                        // P as bf16 hi + lo parts, as in attn_fwd_kernel
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const float e0 = ex2(s[j][0] - mn0), e1 = ex2(s[j][1] - mn0), e2 = ex2(s[j][2] - mn1), e3 = ex2(s[j][3] - mn1);
+            l0 += e0 + e1; l1 += e2 + e3;
+            pr[j][0] = pack_bf16(e0, e1); pr[j][1] = pack_bf16(e2, e3);
+            const float2 h0 = unpack_bf16(pr[j][0]), h1 = unpack_bf16(pr[j][1]);
+            pl[j][0] = pack_bf16(e0 - h0.x, e1 - h0.y); pl[j][1] = pack_bf16(e2 - h1.x, e3 - h1.y);
+        }
+        fence_regs(o);
+        wgmma_fence();
+        wg_pt(o, pr, sV + buf * TILE64_BYTES);
+        wg_pt(o, pl, sV + buf * TILE64_BYTES);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(o); fence_regs(pr); fence_regs(pl);
+        __syncthreads();                                                  // buffer `buf` is refilled at the next iteration
+    }
+    // ---- epilogue: O / l -> ctx, rows below len only
+#pragma unroll
+    for (int off = 1; off < 4; off <<= 1) { l0 += __shfl_xor_sync(0xffffffffu, l0, off); l1 += __shfl_xor_sync(0xffffffffu, l1, off); }
+    const float i0 = 1.0f / l0, i1 = 1.0f / l1;
+    bf16* c0 = p.ctx + (row0 + q0) * p.H + h * HD;
+    bf16* c1 = c0 + 8LL * p.H;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        if (q0 < len) *reinterpret_cast<uint32_t*>(c0 + j * 8 + c) = pack_bf16(o[j][0] * i0, o[j][1] * i0);
+        if (q0 + 8 < len) *reinterpret_cast<uint32_t*>(c1 + j * 8 + c) = pack_bf16(o[j][2] * i1, o[j][3] * i1);
     }
 }
 
@@ -517,6 +645,22 @@ extern "C" int dle_attn_fwd(const void* qkv, const float* mask, void* ctx, float
     int rc = ensure_smem_attr(attn_fwd_kernel, attr, FWD_SMEM_BYTES);
     if (rc != DLE_OK) return rc;
     attn_fwd_kernel<<<dim3(S / FWD_TQ, A, B), FWD_THREADS, FWD_SMEM_BYTES, reinterpret_cast<cudaStream_t>(stream)>>>(p);
+    DLE_LAUNCH_CHECK();
+    return DLE_OK;
+}
+
+extern "C" int dle_attn_fwd_varlen(const void* qkv, const int32_t* cu_seqlens, void* ctx, int32_t B, int32_t max_seqlen, int32_t A,
+                                   void* stream) {
+    DLE_CHECK_ARG(qkv && cu_seqlens && ctx && B > 0 && B <= 65535 && A > 0 && A <= 65535 && max_seqlen >= 1 && max_seqlen <= 512);
+    DLE_CHECK_ARG(aligned16(qkv) && aligned16(ctx) && (reinterpret_cast<uintptr_t>(cu_seqlens) & 3) == 0);
+    VarlenParams p{};
+    p.qkv = reinterpret_cast<const bf16*>(qkv); p.cu_seqlens = cu_seqlens; p.ctx = reinterpret_cast<bf16*>(ctx);
+    p.max_seqlen = max_seqlen; p.H = A * HD; p.scale_log2 = 0.125f * LOG2E;
+    static SmemAttrCache attr;
+    int rc = ensure_smem_attr(attn_fwd_varlen_kernel, attr, FWD_VARLEN_SMEM_BYTES);
+    if (rc != DLE_OK) return rc;
+    attn_fwd_varlen_kernel<<<dim3((max_seqlen + FWD_TQ - 1) / FWD_TQ, A, B), FWD_THREADS, FWD_VARLEN_SMEM_BYTES,
+                             reinterpret_cast<cudaStream_t>(stream)>>>(p);
     DLE_LAUNCH_CHECK();
     return DLE_OK;
 }

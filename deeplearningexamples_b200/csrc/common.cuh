@@ -394,6 +394,11 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[8][4], uint32_t a0
 __device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void* gsrc) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_dst), "l"(gsrc) : "memory");
 }
+// copies src_bytes (0 or 16) from gsrc and zero-fills the rest of the 16 bytes: src_bytes == 0 reads nothing, but gsrc must still
+// be a valid address
+__device__ __forceinline__ void cp_async16_zfill(uint32_t smem_dst, const void* gsrc, uint32_t src_bytes) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_dst), "l"(gsrc), "r"(src_bytes) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ uint4 lds_u4(uint32_t addr) {

@@ -183,8 +183,9 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKernelParams& p, const 
     }
     if (p.epilogue == DLE_EPI_BIAS_GELU) {
         // out2 = pre-activation u (needed by gelu' in backward), out = gelu(u).  gelu is evaluated on the bf16-rounded
-        // pre-activation so that backward (which only has the stored bf16 u) differentiates what forward evaluated.
-        warp_store_rows(p.out2, p.ldo2, row_base, col0, p.M, p.N, stage, lane, v);
+        // pre-activation so that backward (which only has the stored bf16 u) differentiates what forward evaluated.  Inference
+        // passes no out2: u is rounded the same way but not stored.
+        if (p.out2 != nullptr) warp_store_rows(p.out2, p.ldo2, row_base, col0, p.M, p.N, stage, lane, v);
 #pragma unroll
         for (int i = 0; i < 32; i += 2) {
             const uint32_t u2 = pack_bf16(v[i], v[i + 1]);       // the bf16 pair just stored
@@ -500,7 +501,7 @@ extern "C" int dle_gemm_bf16(const dle_gemm_args* a, void* stream_) {
     DLE_CHECK_ARG(a->N % 8 == 0 && a->ldo % 8 == 0 && a->lda % 8 == 0 && a->ldb % 8 == 0);
     DLE_CHECK_ARG(a->epilogue >= 0 && a->epilogue < DLE_EPI_COUNT);
     if (a->epilogue == DLE_EPI_BIAS_DROPOUT_RESIDUAL && a->dropout_p > 0.f) DLE_CHECK_ARG(a->N % 32 == 0);   // 32-element RNG groups
-    if (a->epilogue == DLE_EPI_BIAS_GELU) DLE_CHECK_ARG(a->out2 != nullptr && a->ldo2 % 8 == 0);
+    if (a->epilogue == DLE_EPI_BIAS_GELU && a->out2 != nullptr) DLE_CHECK_ARG(a->ldo2 % 8 == 0);
     if (a->epilogue == DLE_EPI_DGELU || a->epilogue == DLE_EPI_ADD) DLE_CHECK_ARG(a->aux != nullptr);
     if (a->aux != nullptr) DLE_CHECK_ARG(a->ld_aux % 8 == 0 && (reinterpret_cast<uintptr_t>(a->aux) & 15) == 0);
     // the epilogue reads the bias slice with 4- / 8-byte loads and stores 16-byte vectors

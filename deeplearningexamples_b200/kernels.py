@@ -44,7 +44,8 @@ def gemm(a, b, *, a_layout=L.LAYOUT_K, b_layout=L.LAYOUT_K, epilogue=L.EPI_BIAS,
          out=None, out2=None, splits=1, tile_n=0, alpha=1.0, dropout_p=0.0, seed=0, seed_dev=None, dropout_stream=0, colsum_out=None):
     """D[M,N] = alpha * A x B^T with fused epilogue (see include/dle_b200.h).
 
-    a: [M,K] (LAYOUT_K) or [K,M] (LAYOUT_MN);  b: [N,K] (LAYOUT_K) or [K,N] (LAYOUT_MN)."""
+    a: [M,K] (LAYOUT_K) or [K,M] (LAYOUT_MN);  b: [N,K] (LAYOUT_K) or [K,N] (LAYOUT_MN).
+    EPI_BIAS_GELU returns (out, out2 = pre-activation u); out2=False skips the store of u (inference) and returns (out, None)."""
     lib = L.load()
     _req(a, bf16, "A"); _req(b, bf16, "B")
     lda, ldb = _row_major_2d(a, "A"), _row_major_2d(b, "B")
@@ -57,7 +58,11 @@ def gemm(a, b, *, a_layout=L.LAYOUT_K, b_layout=L.LAYOUT_K, epilogue=L.EPI_BIAS,
         out = (torch.zeros if epilogue == L.EPI_ATOMIC_F32 else torch.empty)(
             (M, N), device=a.device, dtype=torch.float32 if f32_out else bf16)
     _req(out, torch.float32 if f32_out else bf16, "out")
-    if epilogue == L.EPI_BIAS_GELU and out2 is None:
+    if out2 is False:
+        if epilogue != L.EPI_BIAS_GELU:
+            raise L.DleError("out2=False applies to EPI_BIAS_GELU only")
+        out2 = None
+    elif epilogue == L.EPI_BIAS_GELU and out2 is None:
         out2 = torch.empty((M, N), device=a.device, dtype=bf16)
     args = L.GemmArgs()
     args.A, args.B, args.out = a.data_ptr(), b.data_ptr(), out.data_ptr()
@@ -98,6 +103,27 @@ def attn_fwd(qkv, mask, B, S, A, dropout_p=0.0, seed=0, dropout_stream=0, seq_fi
     L.launch_count["n"] += 1; L.check(lib.dle_attn_fwd(_ptr(qkv), _ptr(mask), _ptr(ctx), _ptr(lse), B, S, A, 1 if seq_first else 0, dropout_p, seed,
                              _ptr(seed_dev), dropout_stream, _stream()), "dle_attn_fwd")
     return ctx, lse
+
+
+def attn_fwd_varlen(qkv, cu_seqlens, B, max_seqlen, A, out=None):
+    """Inference attention over packed sequences: qkv [T, 3*A*64] bf16, cu_seqlens int32 [B+1] on the device (sequence b is rows
+    cu_seqlens[b] .. cu_seqlens[b+1], each at most max_seqlen <= 512 long).  Returns ctx [T, A*64] (written into `out` when given;
+    rows outside every sequence are left as they are); no mask, dropout or lse."""
+    lib = L.load()
+    _req(qkv, bf16, "qkv"); _req(cu_seqlens, torch.int32, "cu_seqlens")
+    if qkv.dim() != 2 or qkv.shape[1] != 3 * A * 64 or not qkv.is_contiguous():
+        raise L.DleError(f"qkv must be a contiguous [T, {3 * A * 64}] tensor, got shape {tuple(qkv.shape)}")
+    if cu_seqlens.shape != (B + 1,) or not cu_seqlens.is_contiguous():
+        raise L.DleError(f"cu_seqlens must be a contiguous [{B + 1}] tensor, got shape {tuple(cu_seqlens.shape)}")
+    ctx = torch.empty((qkv.shape[0], A * 64), device=qkv.device, dtype=bf16) if out is None else out
+    if ctx.shape != (qkv.shape[0], A * 64) or not ctx.is_contiguous():
+        raise L.DleError(f"out must be a contiguous [{qkv.shape[0]}, {A * 64}] tensor")
+    _req(ctx, bf16, "out")
+    if qkv.shape[0] == 0:
+        return ctx
+    L.launch_count["n"] += 1; L.check(lib.dle_attn_fwd_varlen(_ptr(qkv), _ptr(cu_seqlens), _ptr(ctx), B, max_seqlen, A, _stream()),
+                                      "dle_attn_fwd_varlen")
+    return ctx
 
 
 def attn_bwd(qkv, mask, ctx, dctx, lse, B, S, A, dropout_p=0.0, seed=0, dropout_stream=0, seq_first=False, dbias=None, seed_dev=None):

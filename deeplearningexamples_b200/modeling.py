@@ -30,6 +30,7 @@ from torch.nn.parameter import Parameter
 from torch.utils import checkpoint
 
 from . import _lib as L
+from . import kernels as K
 from . import ops
 
 bf16 = torch.bfloat16
@@ -378,6 +379,18 @@ class BertLayer(nn.Module):
             self.distill_state_dict["hidden_states"] = layer_output
         return layer_output
 
+    def forward_packed(self, x, cu_seqlens, max_seqlen):
+        """Inference forward over packed tokens x [T, H] (BertModel.remove_padding): sequence b is rows cu_seqlens[b] ..
+        cu_seqlens[b+1].  Gives the valid rows of forward's result under a 0 / -10000 mask, with no dropout and no autograd."""
+        if not self._fusable():
+            raise L.DleError("the padding-free route needs the fused layer (head size 64, gelu with bias, no distillation)")
+        att, so, it, out = self.attention.self, self.attention.output, self.intermediate.dense_act, self.output
+        w_qkv, b_qkv = att._packed()
+        return ops.bert_layer_packed_fwd(x, cu_seqlens, max_seqlen, att.num_attention_heads, so.LayerNorm.eps,
+                                         att.query.weight, att.query.bias, so.dense.weight, so.dense.bias, so.LayerNorm.weight,
+                                         so.LayerNorm.bias, it.weight, it.bias, out.dense.weight, out.dense.bias, out.LayerNorm.weight,
+                                         out.LayerNorm.bias, w_qkv, b_qkv)
+
 
 class BertEncoder(nn.Module):
     def __init__(self, config):
@@ -559,6 +572,15 @@ class BertPreTrainedModel(nn.Module):
                 module._checkpoint_activations = val
         self.apply(_apply_flag)
 
+    def remove_padding(self, val):
+        """Padding-free inference (off by default): with it on, an eval-mode forward under torch.no_grad() packs the tokens whose
+        attention_mask is 1 and runs the encoder on those alone (BertModel.forward).  Outputs at masked positions then differ from
+        the padded forward: see BertModel.forward."""
+        def _apply_flag(module):
+            if hasattr(module, "_remove_padding"):
+                module._remove_padding = val
+        self.apply(_apply_flag)
+
     def enable_apex(self, val):
         def _apply_flag(module):
             if hasattr(module, "apex_enabled"):
@@ -648,19 +670,32 @@ class BertModel(BertPreTrainedModel):
         self.apply(self.init_bert_weights)
         self.output_all_encoded_layers = config.output_all_encoded_layers
         self.teacher = False
+        self._remove_padding = False
 
     def forward(self, input_ids, token_type_ids, attention_mask):
+        """With remove_padding(True), an inference call (eval mode, grad disabled; anything else raises) whose attention_mask holds
+        a 0 takes the padding-free route: the positions whose mask is 1 are packed in order, row by row (any 0/1 mask, not only
+        right padding), and the encoder runs on those tokens alone with variable-length attention.  At those positions the outputs
+        equal the padded forward's.  At masked positions every encoded layer is exactly zero (the padded forward computes values
+        there that no consumer should read), and heads see those zero rows; a row with no 1 in its mask is zero throughout (the
+        padded forward averages its values uniformly over the padding there).  The route reads the mask on the host once (one
+        device sync), so it cannot be captured into a CUDA graph.  It takes any S up to 512; the padded path takes S % 128 == 0
+        only.  A batch of such an S without a 0 in its mask, and every call with the switch off, runs the padded path unchanged."""
         if attention_mask is None:
             attention_mask = torch.ones_like(input_ids)
         if token_type_ids is None:
             token_type_ids = torch.zeros_like(input_ids)
-        if self.training:
-            ops.advance_step(input_ids.device)      # fresh dropout masks per forward pass, also when this call is a CUDA-graph replay
-        # additive mask [B,1,1,S]: 0 where attended, -10000 where masked (reference modeling.py:864-872)
-        extended_attention_mask = attention_mask.unsqueeze(1).unsqueeze(2).to(torch.float32)
-        extended_attention_mask = (1.0 - extended_attention_mask) * -10000.0
-        embedding_output = self.embeddings(input_ids, token_type_ids)
-        encoded_layers = self.encoder(embedding_output, extended_attention_mask)
+        packed = self._pack(attention_mask) if self._remove_padding else None
+        if packed is not None:
+            encoded_layers = self._encode_packed(input_ids, token_type_ids, *packed)
+        else:
+            if self.training:
+                ops.advance_step(input_ids.device)  # fresh dropout masks per forward pass, also when this call is a CUDA-graph replay
+            # additive mask [B,1,1,S]: 0 where attended, -10000 where masked (reference modeling.py:864-872)
+            extended_attention_mask = attention_mask.unsqueeze(1).unsqueeze(2).to(torch.float32)
+            extended_attention_mask = (1.0 - extended_attention_mask) * -10000.0
+            embedding_output = self.embeddings(input_ids, token_type_ids)
+            encoded_layers = self.encoder(embedding_output, extended_attention_mask)
         sequence_output = encoded_layers[-1]
         if not self.distillation or (self.distill_config["use_pooler"] and self.distill_config["use_pred_states"]):
             pooled_output = self.pooler(sequence_output)
@@ -670,6 +705,41 @@ class BertModel(BertPreTrainedModel):
             encoded_layers = encoded_layers[-1:]
         if not self.teacher:
             return encoded_layers, pooled_output
+
+    def _pack(self, attention_mask):
+        """(idx, cu_seqlens, T, max_len) of the padding-free route, or None when the mask has no 0 and S % 128 == 0 (the padded
+        path runs)."""
+        if self.training or torch.is_grad_enabled():
+            raise L.DleError("remove_padding(True) is an inference route: call model.eval() and run under torch.no_grad()")
+        B, S = attention_mask.shape
+        keep = attention_mask != 0
+        lens = keep.sum(1, dtype=torch.int32)
+        # the one host read of the route: real token count, longest row and the number of mask values other than 0 and 1
+        T, max_len, bad = torch.stack([lens.sum(), lens.max().long(), (keep & (attention_mask != 1)).sum()]).tolist()
+        if bad:
+            raise L.DleError("attention_mask must hold only 0 and 1 on the padding-free route")
+        if T == B * S and S % 128 == 0:          # no padding, and a length the padded attention takes
+            return None
+        idx = torch.nonzero_static(keep.reshape(-1), size=T).squeeze(-1)
+        cu_seqlens = torch.zeros(B + 1, dtype=torch.int32, device=attention_mask.device)
+        torch.cumsum(lens, 0, dtype=torch.int32, out=cu_seqlens[1:])
+        return idx, cu_seqlens, T, max_len
+
+    def _encode_packed(self, input_ids, token_type_ids, idx, cu_seqlens, T, max_len):
+        """Embeddings + LayerNorm on the padded grid (positions stay the original ones), gather of the kept rows, the encoder layers
+        on the T packed tokens, and scatter back into zeroed [B, S, H] buffers: encoded layers as BertEncoder.forward returns them."""
+        emb = self.embeddings(input_ids, token_type_ids)
+        B, S, H = emb.shape
+        x = K.gather_rows(emb.reshape(B * S, H), idx)
+        encoded_layers = []
+        for layer in self.encoder.layer:
+            if T > 0:
+                x = layer.forward_packed(x, cu_seqlens, max_len)
+            if self.output_all_encoded_layers:
+                encoded_layers.append(K.scatter_rows(x, idx, B * S).view(B, S, H).transpose(0, 1))   # (seq, bsz, hidden) views
+        if not self.output_all_encoded_layers:
+            encoded_layers.append(K.scatter_rows(x, idx, B * S).view(B, S, H))
+        return encoded_layers
 
     def make_teacher(self):
         self.teacher = True

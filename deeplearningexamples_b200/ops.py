@@ -330,6 +330,20 @@ class BertLayerFn(torch.autograd.Function):
                 dwo, c(dbo, bo), c(dg1, g1), c(dbe1, be1), dw1, db1, dw2, c(db2, b2), c(dg2, g2), c(dbe2, be2), None, None, None)
 
 
+def bert_layer_packed_fwd(x, cu_seqlens, max_seqlen, A, eps, wq, bq, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2, w_qkv, b_qkv):
+    """Inference forward of one encoder layer over packed tokens (BertModel.remove_padding): x [T, H], sequence b at rows
+    cu_seqlens[b] .. cu_seqlens[b+1] (int32 [B+1] on the device).  BertLayerFn.forward with the padding removed: variable-length
+    attention instead of a mask, no dropout, no pre-GELU store, no autograd node, nothing saved.  A valid row gets the bits
+    BertLayerFn gives it: the GEMM and LayerNorm results of a row do not depend on the other rows."""
+    qkv = K.gemm(x, w16(w_qkv, key=wq), bias=w16(b_qkv, key=bq))
+    att = K.attn_fwd_varlen(qkv, cu_seqlens, cu_seqlens.numel() - 1, max_seqlen, A)
+    z1 = K.gemm(att, w16(wo), bias=w16(bo), aux=x, epilogue=L.EPI_BIAS_DROPOUT_RESIDUAL)
+    y1 = K.add_ln_fwd(z1, w16(g1), w16(be1), eps=eps)[0]
+    g, _ = K.gemm(y1, w16(w1), bias=w16(b1), epilogue=L.EPI_BIAS_GELU, out2=False)
+    z2 = K.gemm(g, w16(w2), bias=w16(b2), aux=y1, epilogue=L.EPI_BIAS_DROPOUT_RESIDUAL)
+    return K.add_ln_fwd(z2, w16(g2), w16(be2), eps=eps)[0]
+
+
 # -------------------------------------------------------------------------------------------------
 # embeddings: dropout(LayerNorm(word[ids] + pos[arange(S)] + type[tt]))
 # replaces BertEmbeddings.forward (modeling.py:285-301)

@@ -55,7 +55,7 @@ int dle_version(char* host_buf, int host_buf_len);
 #define DLE_LAYOUT_MN 1
 
 #define DLE_EPI_BIAS 0                  /* out = acc (+ bias[n])                        bf16 */
-#define DLE_EPI_BIAS_GELU 1             /* out2 = u = acc + bias; out = gelu_tanh(u)    bf16 */
+#define DLE_EPI_BIAS_GELU 1             /* out2 = u = acc + bias; out = gelu_tanh(u)    bf16 (out2 NULL: u not stored) */
 #define DLE_EPI_BIAS_DROPOUT_RESIDUAL 2 /* out = dropout(acc + bias) + aux              bf16 */
 #define DLE_EPI_DGELU 3                 /* out = acc * gelu_tanh'(aux)                  bf16 */
 #define DLE_EPI_ADD 4                   /* out = acc + aux                              bf16 */
@@ -68,7 +68,7 @@ typedef struct dle_gemm_args {
     const void* A;        /* bf16 */
     const void* B;        /* bf16 */
     void* out;            /* bf16 [M, ldo], or fp32 for DLE_EPI_ATOMIC_F32 / DLE_EPI_F32 */
-    void* out2;           /* bf16 [M, ldo2]: pre-activation for DLE_EPI_BIAS_GELU, else NULL */
+    void* out2;           /* bf16 [M, ldo2]: pre-activation for DLE_EPI_BIAS_GELU (or NULL), else NULL */
     const void* bias;     /* bf16 [N] or NULL */
     const void* aux;      /* bf16 [M, ld_aux]: residual / pre-activation, or NULL */
     int32_t M, N, K;
@@ -101,6 +101,12 @@ int dle_gemm_bf16(const dle_gemm_args* host_args, void* stream);
  * ------------------------------------------------------------------------------------------ */
 int dle_attn_fwd(const void* qkv, const float* mask, void* ctx, float* lse, int32_t B, int32_t S, int32_t A,
                  int32_t seq_first, float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, void* stream);
+/* packed variable-length forward (inference): qkv [T, 3*A*64], ctx [T, A*64], cu_seqlens int32 [B+1] (device, non-decreasing,
+ * cu_seqlens[0] == 0), every length <= max_seqlen <= 512.  No mask, no dropout, no lse.  Sequence b is token rows
+ * cu_seqlens[b] .. cu_seqlens[b+1]; it attends to its own rows only, and only those rows of ctx are written.  A length above
+ * max_seqlen is clamped to max_seqlen; a length of 0 is legal.  A valid row gets the bits dle_attn_fwd gives it in a padded
+ * batch with a -10000 mask on the padding. */
+int dle_attn_fwd_varlen(const void* qkv, const int32_t* cu_seqlens, void* ctx, int32_t B, int32_t max_seqlen, int32_t A, void* stream);
 /* delta_ws: fp32 workspace [B, A, S] (row dots of dO and O); dqkv: bf16 [B*S, 3*A*64], fully overwritten (dQ, dK and dV are
  * each accumulated on chip by exactly one CTA: no atomics, bitwise reproducible);
  * dbias_qkv: fp32 [3*A*64] or NULL: += column sums of dqkv (the q/k/v bias gradients), must be zeroed by the caller */
