@@ -43,6 +43,8 @@ SIGNATURES = {
     "dle_gemm_bf16": (_i32, [ctypes.POINTER(GemmArgs), _vp]),
     "dle_attn_fwd": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _u64, _vp, _u32, _vp]),
     "dle_attn_fwd_varlen": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "dle_attn_fwd_varlen_train": (_i32, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _u64, _vp, _u32, _vp]),
+    "dle_attn_bwd_varlen": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _f32, _u64, _vp, _u32, _vp]),
     "dle_attn_bwd": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _u64, _vp, _u32, _vp]),
     "dle_add_ln_fwd": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _i32, _f32, _f32, _u64, _vp, _u32, _vp]),
     "dle_ln_bwd_partials": (_i32, [_i64]),

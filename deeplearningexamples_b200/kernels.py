@@ -126,6 +126,59 @@ def attn_fwd_varlen(qkv, cu_seqlens, B, max_seqlen, A, out=None):
     return ctx
 
 
+def _check_varlen(qkv, cu_seqlens, B, A):
+    _req(qkv, bf16, "qkv"); _req(cu_seqlens, torch.int32, "cu_seqlens")
+    if qkv.dim() != 2 or qkv.shape[1] != 3 * A * 64 or not qkv.is_contiguous():
+        raise L.DleError(f"qkv must be a contiguous [T, {3 * A * 64}] tensor, got shape {tuple(qkv.shape)}")
+    if cu_seqlens.shape != (B + 1,) or not cu_seqlens.is_contiguous():
+        raise L.DleError(f"cu_seqlens must be a contiguous [{B + 1}] tensor, got shape {tuple(cu_seqlens.shape)}")
+
+
+def _check_rows(t, rows, cols, dtype, name):
+    _req(t, dtype, name)
+    if tuple(t.shape) != (rows, cols) or not t.is_contiguous():
+        raise L.DleError(f"{name} must be a contiguous [{rows}, {cols}] tensor, got shape {tuple(t.shape)}")
+
+
+def attn_fwd_varlen_train(qkv, cu_seqlens, B, max_seqlen, A, drop_stride, dropout_p=0.0, seed=0, dropout_stream=0, seed_dev=None):
+    """Training attention over packed sequences (the arguments of attn_fwd_varlen, plus attn_fwd's dropout).  Returns ctx [T, A*64]
+    and lse fp32 [A, T]; rows outside every sequence are left as they are.  The keep bits of (sequence b, head h, query q, key k) are
+    keyed at ((b*A + h)*drop_stride + q)*drop_stride + k: drop_stride = S (a multiple of 64, max_seqlen <= drop_stride <= 512) draws
+    attn_fwd's bits for a right-padded batch of length S."""
+    lib = L.load()
+    _check_varlen(qkv, cu_seqlens, B, A)
+    T = qkv.shape[0]
+    ctx = torch.empty((T, A * 64), device=qkv.device, dtype=bf16)
+    lse = torch.empty((A, T), device=qkv.device, dtype=torch.float32)
+    if T == 0:
+        return ctx, lse
+    L.launch_count["n"] += 1; L.check(lib.dle_attn_fwd_varlen_train(_ptr(qkv), _ptr(cu_seqlens), _ptr(ctx), _ptr(lse), T, B, max_seqlen, A,
+                                                                    drop_stride, dropout_p, seed, _ptr(seed_dev), dropout_stream, _stream()),
+                                      "dle_attn_fwd_varlen_train")
+    return ctx, lse
+
+
+def attn_bwd_varlen(qkv, cu_seqlens, ctx, dctx, lse, B, max_seqlen, A, drop_stride, dropout_p=0.0, seed=0, dropout_stream=0, dbias=None,
+                    seed_dev=None, out=None):
+    """Backward of attn_fwd_varlen_train: dqkv [T, 3*A*64] (written into `out` when given; rows outside every sequence are left as
+    they are).  dbias: optional zeroed fp32 [3*A*64] receiving the column sums of dqkv's rows inside the sequences."""
+    lib = L.load()
+    _check_varlen(qkv, cu_seqlens, B, A)
+    T, H = qkv.shape[0], A * 64
+    _check_rows(ctx, T, H, bf16, "ctx"); _check_rows(dctx, T, H, bf16, "dctx"); _check_rows(lse, A, T, torch.float32, "lse")
+    dqkv = torch.empty_like(qkv) if out is None else out
+    _check_rows(dqkv, T, 3 * H, bf16, "out")
+    if dbias is not None and (tuple(dbias.shape) != (3 * H,) or not _req(dbias, torch.float32, "dbias").is_contiguous()):
+        raise L.DleError(f"dbias must be a contiguous fp32 [{3 * H}] tensor")
+    if T == 0:
+        return dqkv
+    delta = torch.empty((A, T), device=qkv.device, dtype=torch.float32)
+    L.launch_count["n"] += 3; L.check(lib.dle_attn_bwd_varlen(_ptr(qkv), _ptr(cu_seqlens), _ptr(ctx), _ptr(dctx), _ptr(lse), _ptr(dqkv),
+                                                              _ptr(delta), _ptr(dbias), T, B, max_seqlen, A, drop_stride, dropout_p, seed,
+                                                              _ptr(seed_dev), dropout_stream, _stream()), "dle_attn_bwd_varlen")
+    return dqkv
+
+
 def attn_bwd(qkv, mask, ctx, dctx, lse, B, S, A, dropout_p=0.0, seed=0, dropout_stream=0, seq_first=False, dbias=None, seed_dev=None):
     """dbias: optional zeroed fp32 [3H] receiving the column sums of dqkv (q/k/v bias gradients)."""
     lib = L.load()

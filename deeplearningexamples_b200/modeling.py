@@ -30,7 +30,6 @@ from torch.nn.parameter import Parameter
 from torch.utils import checkpoint
 
 from . import _lib as L
-from . import kernels as K
 from . import ops
 
 bf16 = torch.bfloat16
@@ -87,6 +86,14 @@ def _tokens_like(x, transposed):
     if transposed:
         return x.transpose(0, 1).contiguous().view(-1, H) if not x.transpose(0, 1).is_contiguous() else x.transpose(0, 1).reshape(-1, H)
     return x.contiguous().view(-1, H)
+
+
+def _stream_capturing():
+    """torch.cuda.is_current_stream_capturing(), False where no CUDA device can be used (nothing is capturing there)."""
+    try:
+        return torch.cuda.is_current_stream_capturing()
+    except RuntimeError:
+        return False
 
 
 class LinearActivation(nn.Module):
@@ -379,13 +386,25 @@ class BertLayer(nn.Module):
             self.distill_state_dict["hidden_states"] = layer_output
         return layer_output
 
-    def forward_packed(self, x, cu_seqlens, max_seqlen):
-        """Inference forward over packed tokens x [T, H] (BertModel.remove_padding): sequence b is rows cu_seqlens[b] ..
-        cu_seqlens[b+1].  Gives the valid rows of forward's result under a 0 / -10000 mask, with no dropout and no autograd."""
+    def forward_packed(self, x, cu_seqlens, max_seqlen, drop_stride=None):
+        """Forward over packed tokens x [T, H] (BertModel.remove_padding): sequence b is rows cu_seqlens[b] .. cu_seqlens[b+1].
+        In train mode or with grad enabled, one autograd node (ops.BertLayerPackedFn) with forward's dropout; drop_stride (a multiple
+        of 64 from max_seqlen to 512; the padded length S rounded up to 64) keys the attention masks, so that a right-padded batch draws
+        the padded path's attention keep bits.  Otherwise the inference forward: no dropout and no autograd.  Either way a valid row
+        gets forward's result under a 0 / -10000 mask when dropout is off."""
         if not self._fusable():
             raise L.DleError("the padding-free route needs the fused layer (head size 64, gelu with bias, no distillation)")
         att, so, it, out = self.attention.self, self.attention.output, self.intermediate.dense_act, self.output
         w_qkv, b_qkv = att._packed()
+        if self.training or torch.is_grad_enabled():
+            tr = self.training
+            stride = drop_stride if drop_stride is not None else (max_seqlen + 63) // 64 * 64
+            cfg = (cu_seqlens.numel() - 1, max_seqlen, stride, att.num_attention_heads, att.dropout.p if tr else 0.0,
+                   so.dropout.p if tr else 0.0, so.LayerNorm.eps, att._stream_id, so._stream_id, out._stream_id)
+            return ops.BertLayerPackedFn.apply(x, cu_seqlens, att.query.weight, att.key.weight, att.value.weight, att.query.bias,
+                                               att.key.bias, att.value.bias, so.dense.weight, so.dense.bias, so.LayerNorm.weight,
+                                               so.LayerNorm.bias, it.weight, it.bias, out.dense.weight, out.dense.bias,
+                                               out.LayerNorm.weight, out.LayerNorm.bias, w_qkv, b_qkv, cfg)
         return ops.bert_layer_packed_fwd(x, cu_seqlens, max_seqlen, att.num_attention_heads, so.LayerNorm.eps,
                                          att.query.weight, att.query.bias, so.dense.weight, so.dense.bias, so.LayerNorm.weight,
                                          so.LayerNorm.bias, it.weight, it.bias, out.dense.weight, out.dense.bias, out.LayerNorm.weight,
@@ -572,13 +591,15 @@ class BertPreTrainedModel(nn.Module):
                 module._checkpoint_activations = val
         self.apply(_apply_flag)
 
-    def remove_padding(self, val):
-        """Padding-free inference (off by default): with it on, an eval-mode forward under torch.no_grad() packs the tokens whose
-        attention_mask is 1 and runs the encoder on those alone (BertModel.forward).  Outputs at masked positions then differ from
-        the padded forward: see BertModel.forward."""
+    def remove_padding(self, val, training=False):
+        """Padding-free encoder (off by default): with it on, a forward packs the tokens whose attention_mask is 1 and runs the
+        encoder on those alone (BertModel.forward).  remove_padding(True) is for inference only (eval mode under torch.no_grad());
+        remove_padding(True, training=True) also takes train mode and enabled grad, with autograd through the packed layers.
+        Outputs at masked positions then differ from the padded forward: see BertModel.forward."""
         def _apply_flag(module):
             if hasattr(module, "_remove_padding"):
-                module._remove_padding = val
+                module._remove_padding = bool(val)
+                module._remove_padding_training = bool(val) and bool(training)
         self.apply(_apply_flag)
 
     def enable_apex(self, val):
@@ -671,6 +692,7 @@ class BertModel(BertPreTrainedModel):
         self.output_all_encoded_layers = config.output_all_encoded_layers
         self.teacher = False
         self._remove_padding = False
+        self._remove_padding_training = False
 
     def forward(self, input_ids, token_type_ids, attention_mask):
         """With remove_padding(True), an inference call (eval mode, grad disabled; anything else raises) whose attention_mask holds
@@ -680,7 +702,14 @@ class BertModel(BertPreTrainedModel):
         there that no consumer should read), and heads see those zero rows; a row with no 1 in its mask is zero throughout (the
         padded forward averages its values uniformly over the padding there).  The route reads the mask on the host once (one
         device sync), so it cannot be captured into a CUDA graph.  It takes any S up to 512; the padded path takes S % 128 == 0
-        only.  A batch of such an S without a 0 in its mask, and every call with the switch off, runs the padded path unchanged."""
+        only.  A batch of such an S without a 0 in its mask, and every call with the switch off, runs the padded path unchanged.
+
+        With remove_padding(True, training=True) the route also runs in train mode and with grad enabled: the embeddings (and their
+        dropout) on the padded grid, a row gather to the packed tokens, one autograd node per layer (ops.BertLayerPackedFn) and a
+        row scatter back.  The attention dropout of a right-padded row draws the padded path's keep bits; the dropout of the GEMM
+        epilogues and LayerNorms is keyed by packed position instead.  Masked positions get zero rows and zero gradients, so the
+        pretraining loss is the padded path's whenever every MLM label lies on a kept position and every row keeps position 0.
+        Activation checkpointing is not supported on the route."""
         if attention_mask is None:
             attention_mask = torch.ones_like(input_ids)
         if token_type_ids is None:
@@ -710,7 +739,12 @@ class BertModel(BertPreTrainedModel):
         """(idx, cu_seqlens, T, max_len) of the padding-free route, or None when the mask has no 0 and S % 128 == 0 (the padded
         path runs)."""
         if self.training or torch.is_grad_enabled():
-            raise L.DleError("remove_padding(True) is an inference route: call model.eval() and run under torch.no_grad()")
+            if not self._remove_padding_training:
+                raise L.DleError("remove_padding(True) is an inference route: call model.eval() and run under torch.no_grad()")
+            if _stream_capturing():
+                raise L.DleError("the padding-free route reads the attention mask on the host and cannot be captured into a CUDA graph")
+            if self.encoder._checkpoint_activations:
+                raise L.DleError("the padding-free route does not support activation checkpointing")
         B, S = attention_mask.shape
         keep = attention_mask != 0
         lens = keep.sum(1, dtype=torch.int32)
@@ -728,17 +762,20 @@ class BertModel(BertPreTrainedModel):
     def _encode_packed(self, input_ids, token_type_ids, idx, cu_seqlens, T, max_len):
         """Embeddings + LayerNorm on the padded grid (positions stay the original ones), gather of the kept rows, the encoder layers
         on the T packed tokens, and scatter back into zeroed [B, S, H] buffers: encoded layers as BertEncoder.forward returns them."""
+        if self.training:
+            ops.advance_step(input_ids.device)      # as on the padded path: one bump per training forward
         emb = self.embeddings(input_ids, token_type_ids)
         B, S, H = emb.shape
-        x = K.gather_rows(emb.reshape(B * S, H), idx)
+        x = ops.GatherRowsFn.apply(emb.reshape(B * S, H), idx)
+        drop_stride = (S + 63) // 64 * 64       # attention dropout keyed as on the padded [B, S] grid
         encoded_layers = []
         for layer in self.encoder.layer:
             if T > 0:
-                x = layer.forward_packed(x, cu_seqlens, max_len)
+                x = layer.forward_packed(x, cu_seqlens, max_len, drop_stride)
             if self.output_all_encoded_layers:
-                encoded_layers.append(K.scatter_rows(x, idx, B * S).view(B, S, H).transpose(0, 1))   # (seq, bsz, hidden) views
+                encoded_layers.append(ops.ScatterRowsFn.apply(x, idx, B * S).view(B, S, H).transpose(0, 1))   # (seq, bsz, hidden) views
         if not self.output_all_encoded_layers:
-            encoded_layers.append(K.scatter_rows(x, idx, B * S).view(B, S, H))
+            encoded_layers.append(ops.ScatterRowsFn.apply(x, idx, B * S).view(B, S, H))
         return encoded_layers
 
     def make_teacher(self):

@@ -273,61 +273,111 @@ class BertLayerFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, mask, wq, wk, wv, bq, bk, bv, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2, w_qkv, b_qkv, cfg):
         B, S, A, p_attn, p_hid, eps, sid_attn, sid_h1, sid_h2, seq_first = cfg
-        seed_a = next_seed() if p_attn > 0.0 else 0
-        seed_1 = next_seed() if p_hid > 0.0 else 0
-        seed_2 = next_seed() if p_hid > 0.0 else 0
-        sdev = step_counter(x.device)
-        qkv = K.gemm(x, w16(w_qkv, key=wq), bias=w16(b_qkv, key=bq))
-        att, lse = K.attn_fwd(qkv, mask, B, S, A, dropout_p=p_attn, seed=seed_a, dropout_stream=sid_attn, seq_first=seq_first, seed_dev=sdev)
-        z1 = K.gemm(att, w16(wo), bias=w16(bo), aux=x, epilogue=L.EPI_BIAS_DROPOUT_RESIDUAL, dropout_p=p_hid, seed=seed_1,
-                    dropout_stream=sid_h1, seed_dev=sdev)
-        y1, _, mean1, rstd1 = K.add_ln_fwd(z1, w16(g1), w16(be1), eps=eps)
-        g, u = K.gemm(y1, w16(w1), bias=w16(b1), epilogue=L.EPI_BIAS_GELU)
-        z2 = K.gemm(g, w16(w2), bias=w16(b2), aux=y1, epilogue=L.EPI_BIAS_DROPOUT_RESIDUAL, dropout_p=p_hid, seed=seed_2,
-                    dropout_stream=sid_h2, seed_dev=sdev)
-        y2, _, mean2, rstd2 = K.add_ln_fwd(z2, w16(g2), w16(be2), eps=eps)
-        ctx.save_for_backward(x, mask, qkv, att, lse, z1, mean1, rstd1, y1, u, g, z2, mean2, rstd2, w_qkv)
-        ctx.params = (wq, bq, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2)
         ctx.cfg = cfg
-        ctx.seeds = (seed_a, seed_1, seed_2)
-        return y2
+
+        def attn(qkv, seed_a, sdev):
+            return K.attn_fwd(qkv, mask, B, S, A, dropout_p=p_attn, seed=seed_a, dropout_stream=sid_attn, seq_first=seq_first, seed_dev=sdev)
+        return _layer_forward(ctx, x, mask, attn, (wq, bq, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2), w_qkv, b_qkv, p_attn, p_hid, eps,
+                              sid_h1, sid_h2)
 
     @staticmethod
     def backward(ctx, dy2):
-        x, mask, qkv, att, lse, z1, mean1, rstd1, y1, u, g, z2, mean2, rstd2, w_qkv = ctx.saved_tensors
-        wq, bq, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2 = ctx.params
         B, S, A, p_attn, p_hid, eps, sid_attn, sid_h1, sid_h2, seq_first = ctx.cfg
-        seed_a, seed_1, seed_2 = ctx.seeds
-        H_ = x.shape[1]
-        sdev = step_counter(x.device)
-        # bias gradients of FFN1 (4H) and q|k|v (3H) are column sums of tensors produced below: the producing kernels accumulate
-        # them (warp transpose-reduce + red.add) instead of a separate pass re-reading du / dqkv from HBM
-        bias_acc = torch.zeros(w1.shape[0] + 3 * H_, device=x.device, dtype=torch.float32)
-        db1_acc, dbqkv_acc = bias_acc[:w1.shape[0]], bias_acc[w1.shape[0]:]
-        # ---- BertOutput
-        dz2, dh2, dg2, dbe2, db2 = K.add_ln_bwd(dy2.contiguous(), z2, mean2, rstd2, w16(g2), dropout_p=p_hid, seed=seed_2,
-                                                dropout_stream=sid_h2, out_dtype=g2.dtype, seed_dev=sdev)
-        du = K.gemm(dh2, w16(w2), b_layout=L.LAYOUT_MN, epilogue=L.EPI_DGELU, aux=u, colsum_out=db1_acc)   # dgrad * gelu'(u)
-        dw2 = wgrad(dh2, g, w2.dtype)
-        # ---- BertIntermediate (+ residual branch of BertOutput folded into the epilogue)
-        dy1 = K.gemm(du, w16(w1), b_layout=L.LAYOUT_MN, epilogue=L.EPI_ADD, aux=dz2)
-        dw1 = wgrad(du, y1, w1.dtype)
-        # ---- BertSelfOutput
-        dz1, dh1, dg1, dbe1, dbo = K.add_ln_bwd(dy1, z1, mean1, rstd1, w16(g1), dropout_p=p_hid, seed=seed_1, dropout_stream=sid_h1,
-                                                out_dtype=g1.dtype, seed_dev=sdev)
-        datt = K.gemm(dh1, w16(wo), b_layout=L.LAYOUT_MN)
-        dwo = wgrad(dh1, att, wo.dtype)
-        # ---- BertSelfAttention (+ residual branch of BertSelfOutput folded into the QKV dgrad epilogue)
-        dqkv = K.attn_bwd(qkv, mask, att, datt, lse, B, S, A, dropout_p=p_attn, seed=seed_a, dropout_stream=sid_attn, seq_first=seq_first,
-                          dbias=dbqkv_acc, seed_dev=sdev)
-        dx = K.gemm(dqkv, w16(w_qkv, key=wq), b_layout=L.LAYOUT_MN, epilogue=L.EPI_ADD, aux=dz1)
-        dwqkv = wgrad(dqkv, x, wq.dtype)
-        bias_g = bias_acc if b1.dtype == torch.float32 else bias_acc.to(b1.dtype)
-        db1, dbqkv = bias_g[:w1.shape[0]], bias_g[w1.shape[0]:]
-        H = dwqkv.shape[1]
-        c = _to_param_dtype
-        return (dx, None, dwqkv[0:H], dwqkv[H:2 * H], dwqkv[2 * H:3 * H], dbqkv[0:H], dbqkv[H:2 * H], dbqkv[2 * H:3 * H],
-                dwo, c(dbo, bo), c(dg1, g1), c(dbe1, be1), dw1, db1, dw2, c(db2, b2), c(dg2, g2), c(dbe2, be2), None, None, None)
+
+        def attn_bwd(qkv, mask, att, datt, lse, seed_a, dbias, sdev):
+            return K.attn_bwd(qkv, mask, att, datt, lse, B, S, A, dropout_p=p_attn, seed=seed_a, dropout_stream=sid_attn,
+                              seq_first=seq_first, dbias=dbias, seed_dev=sdev)
+        return _layer_backward(ctx, dy2, attn_bwd, p_hid, sid_h1, sid_h2)
+
+
+# -------------------------------------------------------------------------------------------------
+# the encoder layer over packed tokens (BertModel.remove_padding in training): BertLayerFn with variable-length attention
+# -------------------------------------------------------------------------------------------------
+class BertLayerPackedFn(torch.autograd.Function):
+    """BertLayerFn over packed tokens x [T, H]: sequence b is rows cu_seqlens[b] .. cu_seqlens[b+1] (int32 [B+1] on the device).  The
+    same GEMM, LayerNorm and epilogue calls on T rows, the same saved tensors (lse is [A, T]), the same seed draws and stream ids.  With
+    drop_stride = S the attention keep bits are those BertLayerFn draws for a right-padded batch of length S; the GEMM-epilogue and
+    LayerNorm dropout masks are keyed by element index in the packed tensors, so they differ from the padded path's.
+    cfg = (B, max_seqlen, drop_stride, A, p_attn, p_hid, eps, sid_attn, sid_h1, sid_h2)."""
+
+    @staticmethod
+    def forward(ctx, x, cu_seqlens, wq, wk, wv, bq, bk, bv, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2, w_qkv, b_qkv, cfg):
+        B, max_seqlen, drop_stride, A, p_attn, p_hid, eps, sid_attn, sid_h1, sid_h2 = cfg
+        ctx.cfg = cfg
+
+        def attn(qkv, seed_a, sdev):
+            return K.attn_fwd_varlen_train(qkv, cu_seqlens, B, max_seqlen, A, drop_stride, dropout_p=p_attn, seed=seed_a,
+                                           dropout_stream=sid_attn, seed_dev=sdev)
+        return _layer_forward(ctx, x, cu_seqlens, attn, (wq, bq, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2), w_qkv, b_qkv, p_attn, p_hid,
+                              eps, sid_h1, sid_h2)
+
+    @staticmethod
+    def backward(ctx, dy2):
+        B, max_seqlen, drop_stride, A, p_attn, p_hid, eps, sid_attn, sid_h1, sid_h2 = ctx.cfg
+
+        def attn_bwd(qkv, cu_seqlens, att, datt, lse, seed_a, dbias, sdev):
+            return K.attn_bwd_varlen(qkv, cu_seqlens, att, datt, lse, B, max_seqlen, A, drop_stride, dropout_p=p_attn, seed=seed_a,
+                                     dropout_stream=sid_attn, dbias=dbias, seed_dev=sdev)
+        return _layer_backward(ctx, dy2, attn_bwd, p_hid, sid_h1, sid_h2)
+
+
+def _layer_forward(ctx, x, attn_aux, attn, params, w_qkv, b_qkv, p_attn, p_hid, eps, sid_h1, sid_h2):
+    """Forward of BertLayerFn / BertLayerPackedFn.  attn(qkv, seed, seed_dev) -> (ctx, lse) is the layer's attention; attn_aux (mask
+    or cu_seqlens) is saved for its backward."""
+    wq, bq, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2 = params
+    seed_a = next_seed() if p_attn > 0.0 else 0
+    seed_1 = next_seed() if p_hid > 0.0 else 0
+    seed_2 = next_seed() if p_hid > 0.0 else 0
+    sdev = step_counter(x.device)
+    qkv = K.gemm(x, w16(w_qkv, key=wq), bias=w16(b_qkv, key=bq))
+    att, lse = attn(qkv, seed_a, sdev)
+    z1 = K.gemm(att, w16(wo), bias=w16(bo), aux=x, epilogue=L.EPI_BIAS_DROPOUT_RESIDUAL, dropout_p=p_hid, seed=seed_1,
+                dropout_stream=sid_h1, seed_dev=sdev)
+    y1, _, mean1, rstd1 = K.add_ln_fwd(z1, w16(g1), w16(be1), eps=eps)
+    g, u = K.gemm(y1, w16(w1), bias=w16(b1), epilogue=L.EPI_BIAS_GELU)
+    z2 = K.gemm(g, w16(w2), bias=w16(b2), aux=y1, epilogue=L.EPI_BIAS_DROPOUT_RESIDUAL, dropout_p=p_hid, seed=seed_2,
+                dropout_stream=sid_h2, seed_dev=sdev)
+    y2, _, mean2, rstd2 = K.add_ln_fwd(z2, w16(g2), w16(be2), eps=eps)
+    ctx.save_for_backward(x, attn_aux, qkv, att, lse, z1, mean1, rstd1, y1, u, g, z2, mean2, rstd2, w_qkv)
+    ctx.params = params
+    ctx.seeds = (seed_a, seed_1, seed_2)
+    return y2
+
+
+def _layer_backward(ctx, dy2, attn_bwd, p_hid, sid_h1, sid_h2):
+    """Backward of BertLayerFn / BertLayerPackedFn.  attn_bwd(qkv, attn_aux, ctx, dctx, lse, seed, dbias, seed_dev) -> dqkv."""
+    x, attn_aux, qkv, att, lse, z1, mean1, rstd1, y1, u, g, z2, mean2, rstd2, w_qkv = ctx.saved_tensors
+    wq, bq, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2 = ctx.params
+    seed_a, seed_1, seed_2 = ctx.seeds
+    H_ = x.shape[1]
+    sdev = step_counter(x.device)
+    # bias gradients of FFN1 (4H) and q|k|v (3H) are column sums of tensors produced below: the producing kernels accumulate
+    # them (warp transpose-reduce + red.add) instead of a separate pass re-reading du / dqkv from HBM
+    bias_acc = torch.zeros(w1.shape[0] + 3 * H_, device=x.device, dtype=torch.float32)
+    db1_acc, dbqkv_acc = bias_acc[:w1.shape[0]], bias_acc[w1.shape[0]:]
+    # ---- BertOutput
+    dz2, dh2, dg2, dbe2, db2 = K.add_ln_bwd(dy2.contiguous(), z2, mean2, rstd2, w16(g2), dropout_p=p_hid, seed=seed_2,
+                                            dropout_stream=sid_h2, out_dtype=g2.dtype, seed_dev=sdev)
+    du = K.gemm(dh2, w16(w2), b_layout=L.LAYOUT_MN, epilogue=L.EPI_DGELU, aux=u, colsum_out=db1_acc)   # dgrad * gelu'(u)
+    dw2 = wgrad(dh2, g, w2.dtype)
+    # ---- BertIntermediate (+ residual branch of BertOutput folded into the epilogue)
+    dy1 = K.gemm(du, w16(w1), b_layout=L.LAYOUT_MN, epilogue=L.EPI_ADD, aux=dz2)
+    dw1 = wgrad(du, y1, w1.dtype)
+    # ---- BertSelfOutput
+    dz1, dh1, dg1, dbe1, dbo = K.add_ln_bwd(dy1, z1, mean1, rstd1, w16(g1), dropout_p=p_hid, seed=seed_1, dropout_stream=sid_h1,
+                                            out_dtype=g1.dtype, seed_dev=sdev)
+    datt = K.gemm(dh1, w16(wo), b_layout=L.LAYOUT_MN)
+    dwo = wgrad(dh1, att, wo.dtype)
+    # ---- BertSelfAttention (+ residual branch of BertSelfOutput folded into the QKV dgrad epilogue)
+    dqkv = attn_bwd(qkv, attn_aux, att, datt, lse, seed_a, dbqkv_acc, sdev)
+    dx = K.gemm(dqkv, w16(w_qkv, key=wq), b_layout=L.LAYOUT_MN, epilogue=L.EPI_ADD, aux=dz1)
+    dwqkv = wgrad(dqkv, x, wq.dtype)
+    bias_g = bias_acc if b1.dtype == torch.float32 else bias_acc.to(b1.dtype)
+    db1, dbqkv = bias_g[:w1.shape[0]], bias_g[w1.shape[0]:]
+    H = dwqkv.shape[1]
+    c = _to_param_dtype
+    return (dx, None, dwqkv[0:H], dwqkv[H:2 * H], dwqkv[2 * H:3 * H], dbqkv[0:H], dbqkv[H:2 * H], dbqkv[2 * H:3 * H],
+            dwo, c(dbo, bo), c(dg1, g1), c(dbe1, be1), dw1, db1, dw2, c(db2, b2), c(dg2, g2), c(dbe2, be2), None, None, None)
 
 
 def bert_layer_packed_fwd(x, cu_seqlens, max_seqlen, A, eps, wq, bq, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2, w_qkv, b_qkv):
@@ -400,6 +450,20 @@ class GatherRowsFn(torch.autograd.Function):
     def backward(ctx, dy):
         (idx,) = ctx.saved_tensors
         return K.scatter_rows(dy.contiguous(), idx, ctx.n_rows), None
+
+
+class ScatterRowsFn(torch.autograd.Function):
+    """out[idx[i]] = x[i] in a zeroed [n_rows, H] tensor (the packed tokens back onto the padded grid); backward gathers the rows."""
+
+    @staticmethod
+    def forward(ctx, x, idx, n_rows):
+        ctx.save_for_backward(idx)
+        return K.scatter_rows(x, idx, n_rows)
+
+    @staticmethod
+    def backward(ctx, dy):
+        (idx,) = ctx.saved_tensors
+        return K.gather_rows(dy.contiguous(), idx, err_flag=err_flag(dy.device)), None, None
 
 
 # -------------------------------------------------------------------------------------------------

@@ -13,6 +13,9 @@ What is different, and why:
   * TorchScript is not applicable to custom autograd functions: `--disable_jit_fusions` is implied.
   * `--cuda_graphs` captures the whole step (and the gradient-accumulation micro-step) exactly as the reference does (:602-640,669);
     dropout stays on: masks are keyed by a device-side step counter (ops.step_counter) that the captured forward bumps.
+  * `--remove_padding` (not in the reference) trains padding-free: every encoder layer runs on the real tokens of the batch only
+    (BertModel.remove_padding(True, training=True)).  It reads each batch's mask on the host, so it excludes `--cuda_graphs`, and it
+    excludes `--checkpoint_activations`.
 """
 import argparse
 import json
@@ -127,7 +130,12 @@ def parse_arguments(argv=None):
     p.add_argument("--no_dense_sequence_output", default=False, action="store_true")
     p.add_argument("--disable_jit_fusions", default=False, action="store_true")
     p.add_argument("--cuda_graphs", default=False, action="store_true")
+    p.add_argument("--remove_padding", default=False, action="store_true",
+                   help="padding-free training: run the encoder on the real tokens of each batch only (BertModel.remove_padding)")
     args = p.parse_args(argv)
+    if args.remove_padding and (args.cuda_graphs or args.checkpoint_activations):
+        raise ValueError("--remove_padding reads each batch's attention mask on the host: it cannot be combined with --cuda_graphs, "
+                         "and the padding-free encoder does not support --checkpoint_activations")
     args.fp16 = args.fp16 or args.amp
     args.local_rank = int(args.local_rank)
     if args.steps_this_run < 0:
@@ -206,6 +214,8 @@ def prepare_model_and_optimizer(args, device, sequence_output_is_dense):
                                        base_lr=args.learning_rate, device=device)
     grad_scaler = torch.amp.GradScaler("cuda", init_scale=args.init_loss_scale, enabled=args.fp16)
     model.checkpoint_activations(args.checkpoint_activations)
+    if args.remove_padding:
+        model.remove_padding(True, training=True)
     if args.resume_from_checkpoint:
         if (args.phase2 and not args.resume_phase2) or args.init_checkpoint:
             for group in checkpoint['optimizer']['param_groups']:       # new phase: restart the schedule

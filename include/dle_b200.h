@@ -107,12 +107,28 @@ int dle_attn_fwd(const void* qkv, const float* mask, void* ctx, float* lse, int3
  * max_seqlen is clamped to max_seqlen; a length of 0 is legal.  A valid row gets the bits dle_attn_fwd gives it in a padded
  * batch with a -10000 mask on the padding. */
 int dle_attn_fwd_varlen(const void* qkv, const int32_t* cu_seqlens, void* ctx, int32_t B, int32_t max_seqlen, int32_t A, void* stream);
+/* packed variable-length forward for training: dle_attn_fwd_varlen plus dle_attn_fwd's dropout, and lse fp32 [A, T] (head h, token
+ * row t at h*T + t; rows outside every sequence are not written).  cu_seqlens[B] <= T.  The Philox block of (sequence b, head h,
+ * in-sequence query q, in-sequence key k) is drawn at ((b*A + h)*drop_stride + q)*drop_stride + k, drop_stride a multiple of 64 with
+ * max_seqlen <= drop_stride <= 512: with drop_stride = S a right-padded batch draws dle_attn_fwd's keep bits, and a valid row gets
+ * dle_attn_fwd's bits (ctx and lse) under a -10000 mask on the padding. */
+int dle_attn_fwd_varlen_train(const void* qkv, const int32_t* cu_seqlens, void* ctx, float* lse, int32_t T, int32_t B,
+                              int32_t max_seqlen, int32_t A, int32_t drop_stride, float dropout_p, uint64_t seed,
+                              const uint64_t* seed_dev, uint32_t dropout_stream, void* stream);
 /* delta_ws: fp32 workspace [B, A, S] (row dots of dO and O); dqkv: bf16 [B*S, 3*A*64], fully overwritten (dQ, dK and dV are
  * each accumulated on chip by exactly one CTA: no atomics, bitwise reproducible);
  * dbias_qkv: fp32 [3*A*64] or NULL: += column sums of dqkv (the q/k/v bias gradients), must be zeroed by the caller */
 int dle_attn_bwd(const void* qkv, const float* mask, const void* ctx, const void* dctx, const float* lse,
                  void* dqkv, float* delta_ws, float* dbias_qkv, int32_t B, int32_t S, int32_t A, int32_t seq_first, float dropout_p,
                  uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, void* stream);
+/* packed variable-length backward: the arguments of dle_attn_fwd_varlen_train, with delta_ws fp32 [A, T].  Only the rows of dqkv
+ * inside a sequence are written (each by exactly one CTA, as in dle_attn_bwd), and dbias_qkv (zeroed by the caller, or NULL) receives
+ * the column sums of those rows only.  With drop_stride = S, the valid rows of a right-padded batch get dle_attn_bwd's bits when dctx
+ * is 0 on the padding. */
+int dle_attn_bwd_varlen(const void* qkv, const int32_t* cu_seqlens, const void* ctx, const void* dctx, const float* lse,
+                        void* dqkv, float* delta_ws, float* dbias_qkv, int32_t T, int32_t B, int32_t max_seqlen, int32_t A,
+                        int32_t drop_stride, float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream,
+                        void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * (bias +) dropout + residual-add + LayerNorm, vectorised warp-shuffle kernels (HBM-bound)
