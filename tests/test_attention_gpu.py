@@ -151,8 +151,9 @@ def test_attention_linear_in_v_full_size():
 
 
 def test_attention_skips_fully_padded_key_tiles():
-    """Variable-length batches (SURVEY.md 8f rank 3): key tiles whose additive mask is -10000 for every key are skipped outright by
-    the kernels; the results must equal the dense computation (fp32 reference) and dK / dV of padded keys must be exactly zero."""
+    """Variable-length batches (SURVEY.md 8f rank 3) with whole key tiles under a -10000 mask.  The padded kernels visit every key
+    tile (DESIGN.md); this checks that lse, ctx and dqkv still match the fp32 reference, that dK / dV of padded keys are exactly zero,
+    and that a padded row gives the same bits alone as inside a batch with longer rows."""
     k = _k()
     B, S, A = 4, 512, 2
     H = A * 64
