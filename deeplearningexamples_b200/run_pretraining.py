@@ -284,6 +284,27 @@ def take_optimizer_step(args, lr_scheduler, optimizer, grad_scaler, skipped_acc)
     optimizer.zero_grad(set_to_none=not (args.cuda_graphs and args.gradient_accumulation_steps > 1))
 
 
+def capture_training_graphs(args, model, optimizer, grad_scaler, lr_scheduler, criterion, static_batch, loss_acc, skipped_acc):
+    """reference :602-640: eager warm-up on a side stream, then one captured graph for the full step (micro-step + optimizer step) and,
+    with gradient accumulation, one for the micro-step alone (no_sync under DDP).  Both read `static_batch`, which must hold a real
+    batch (all-ones labels, as the reference uses, would mark every position as masked and trip the static masked-row bound), and add
+    into `loss_acc` / `skipped_acc`.  The warm-ups train on the static batch, as the reference's do.  Returns (full_graph, accum_graph);
+    accum_graph is None without gradient accumulation."""
+    full_graph = capture_step_graph(lambda: (take_training_step(args, grad_scaler, model, criterion, static_batch, loss_acc),
+                                             take_optimizer_step(args, lr_scheduler, optimizer, grad_scaler, skipped_acc)), warmup_iters=11)
+    accum_graph = None
+    if args.gradient_accumulation_steps > 1:
+        def micro():
+            if hasattr(model, "no_sync"):
+                with model.no_sync():
+                    take_training_step(args, grad_scaler, model, criterion, static_batch, loss_acc)
+            else:
+                take_training_step(args, grad_scaler, model, criterion, static_batch, loss_acc)
+        accum_graph = capture_step_graph(micro, warmup_iters=3)
+        optimizer.zero_grad(set_to_none=False)       # the warm-up / captured micro-steps accumulated into the static gradient buffers
+    return full_graph, accum_graph
+
+
 def main(argv=None):
     global timeout_sent
     signal.signal(signal.SIGTERM, _on_sigterm)
@@ -324,22 +345,10 @@ def main(argv=None):
     skip_for_perf = 50 if args.phase2 else 4
     static_batch = full_graph = accum_graph = None
     if args.cuda_graphs:
-        # reference :602-640: a static device batch, eager warm-up on a side stream, then one captured graph for the full step and one
-        # for the gradient-accumulation micro-step (no_sync under DDP).  The static batch starts as a real batch (all-ones labels, as
-        # the reference uses, would mark every position as masked and trip the static masked-row bound).
         first = next(iter(loader))
         static_batch = {k: v.to(device) for k, v in first.items()}
-        full_graph = capture_step_graph(lambda: (take_training_step(args, grad_scaler, model, criterion, static_batch, loss_acc),
-                                                 take_optimizer_step(args, lr_scheduler, optimizer, grad_scaler, skipped_acc)), warmup_iters=11)
-        if args.gradient_accumulation_steps > 1:
-            def micro():
-                if hasattr(model, "no_sync"):
-                    with model.no_sync():
-                        take_training_step(args, grad_scaler, model, criterion, static_batch, loss_acc)
-                else:
-                    take_training_step(args, grad_scaler, model, criterion, static_batch, loss_acc)
-            accum_graph = capture_step_graph(micro, warmup_iters=3)
-            optimizer.zero_grad(set_to_none=False)       # the warm-up / captured micro-steps accumulated into the static gradient buffers
+        full_graph, accum_graph = capture_training_graphs(args, model, optimizer, grad_scaler, lr_scheduler, criterion, static_batch,
+                                                          loss_acc, skipped_acc)
         # the warm-up / capture executions advanced the optimizer: rewind the statistics the run reports (weights keep the 12+ steps,
         # exactly as in the reference, whose warm-up also trains on the static batch)
         loss_acc.zero_()

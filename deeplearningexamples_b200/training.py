@@ -150,6 +150,9 @@ def capture_step_graph(fn, warmup_iters=11):
         for _ in range(warmup_iters):
             fn()
     torch.cuda.current_stream().wait_stream(side)
+    # fp32 parameters: the graph must contain the bf16 casts it reads (ops.w16).  A copy the warm-ups cached is valid now, but a
+    # replay that reused it would read the weights of capture time on every replay, however the optimizer changed them since.
+    ops.weight_epoch["n"] += 1
     graph = torch.cuda.CUDAGraph()
     # thread_local: CUDA calls made by OTHER host threads during the capture (NCCL watchdog, data-loader pinning) must not invalidate it
     with torch.cuda.graph(graph, capture_error_mode="thread_local"):

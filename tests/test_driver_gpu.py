@@ -53,3 +53,12 @@ def test_gradient_accumulation_matches_reference_batch_split(tmp_path):
     """train_batch_size is divided by the accumulation steps (:363); 2 micro-steps of 2 == 1 optimizer step."""
     args, t_raw, model_step, *_ = _run(tmp_path, ["--max_steps", "3", "--gradient_accumulation_steps", "2", "--skip_checkpoint"])
     assert args.train_batch_size == 2 and model_step == 6
+
+
+def test_gradient_accumulation_under_cuda_graphs(tmp_path):
+    """The same batch split with --cuda_graphs: the micro-steps replay the accumulation graph, every second step the full-step graph.
+    The capture's 14 warm-ups take optimizer steps, so the schedule runs past them (--max_steps 100); the run stops after 3 steps."""
+    args, t_raw, model_step, skip, final_loss, _ = _run(tmp_path, ["--max_steps", "100", "--steps_this_run", "3", "--cuda_graphs",
+                                                                   "--gradient_accumulation_steps", "2", "--skip_checkpoint"])
+    assert args.train_batch_size == 2 and model_step == 6
+    assert 0.0 < final_loss < 12.0
