@@ -537,7 +537,8 @@ embed_ln_fwd_kernel(const long long* __restrict__ ids, const long long* __restri
                     const bf16* __restrict__ pos, const bf16* __restrict__ type, const bf16* __restrict__ gamma,
                     const bf16* __restrict__ beta, bf16* __restrict__ z_out, bf16* __restrict__ y, float* __restrict__ mean_out,
                     float* __restrict__ rstd_out, int B, int S, int V, int P, int NT, float eps, uint32_t thresh,
-                    float drop_scale, unsigned long long seed, const unsigned long long* seed_dev, uint32_t stream_id, int* err_flag) {
+                    float drop_scale, unsigned long long seed, const unsigned long long* seed_dev, uint32_t stream_id, int* err_flag,
+                    const long long* __restrict__ pos_ids) {
     seed = effective_seed(seed, seed_dev);
     constexpr int H = J * 256;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -550,11 +551,12 @@ embed_ln_fwd_kernel(const long long* __restrict__ ids, const long long* __restri
     }
     for (long long row = (long long)blockIdx.x * LN_WARPS + warp; row < T; row += (long long)gridDim.x * LN_WARPS) {
         long long id = ids[row], tt = tts[row];
-        const int s = (int)(row % S);
-        if (id < 0 || id >= V || tt < 0 || tt >= NT || s >= P) {
+        long long sp = pos_ids ? pos_ids[row] : row % S;         // explicit positions restart per packed sample
+        if (id < 0 || id >= V || tt < 0 || tt >= NT || sp < 0 || sp >= P) {
             if (err_flag && lane == 0) atomicExch(err_flag, 1);
-            id = 0; tt = 0;
+            id = 0; tt = 0; sp = 0;
         }
+        const int s = (int)sp;
         float z[J * 8];
 #pragma unroll
         for (int j = 0; j < J; ++j) {
@@ -592,7 +594,8 @@ embed_ln_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ z, con
                     const float* __restrict__ rstd_in, const bf16* __restrict__ gamma, const long long* __restrict__ ids,
                     const long long* __restrict__ tts, float* __restrict__ dword, float* __restrict__ dpos,
                     float* __restrict__ dtype_tab, float* __restrict__ part_dgamma, float* __restrict__ part_dbeta,
-                    int B, int S, uint32_t thresh, float drop_scale, unsigned long long seed, const unsigned long long* seed_dev, uint32_t stream_id) {
+                    int B, int S, uint32_t thresh, float drop_scale, unsigned long long seed, const unsigned long long* seed_dev, uint32_t stream_id,
+                    const long long* __restrict__ pos_ids) {
     seed = effective_seed(seed, seed_dev);
     constexpr int H = J * 256;
     __shared__ float red[LN_WARPS][H];
@@ -632,7 +635,7 @@ embed_ln_bwd_kernel(const bf16* __restrict__ dy, const bf16* __restrict__ z, con
         }
         s1 = warp_sum(s1) * invH; s2 = warp_sum(s2) * invH;
         const long long id = ids[row], tt = tts[row];
-        const int s = (int)(row % S);
+        const int s = (int)(pos_ids ? pos_ids[row] : row % S);
 #pragma unroll
         for (int j = 0; j < J; ++j) {
             const int col = j * 256 + lane * 8;
@@ -693,6 +696,78 @@ __global__ void scatter_rows_kernel(const bf16* __restrict__ dy, const long long
         if (dst < 0 || dst >= n_rows) continue;
         *reinterpret_cast<uint4*>(dx + dst * H + c * 8) = ld_global_nc_v4(dy + r * H + c * 8);
     }
+}
+// ---------------------------------------------------------------------------------------------
+// segment table of a packed batch: mask[b, s] = sample number j (1..k, contiguous, increasing), 0 on the row's padding tail
+// ---------------------------------------------------------------------------------------------
+constexpr int SEG_WARPS = 4;
+
+// one warp per row, two passes over the row in 32-token chunks: (1) validate and find the row's real-token count n and sample count m,
+// (2) write positions, segment starts and [CLS] rows.  A malformed row is written as if its mask were all 0 (one tail segment).
+__global__ void __launch_bounds__(SEG_WARPS * 32)
+segment_table_kernel(const long long* __restrict__ mask, int B, int S, int k, int* __restrict__ cu_seqlens,
+                     long long* __restrict__ position_ids, long long* __restrict__ cls_index, int* err_flag) {
+    const int lane = threadIdx.x & 31;
+    const int b = blockIdx.x * SEG_WARPS + (threadIdx.x >> 5);
+    if (b >= B) return;
+    const long long* m_row = mask + (long long)b * S;
+    const long long row0 = (long long)b * S;
+    // pass 1: every token must satisfy 0 <= v <= k and v == 0 || (s == 0 ? v == 1 : prev != 0 && (v == prev || v == prev + 1))
+    bool bad = false;
+    int n = 0, m = 0;
+    long long carry = 0;                                     // value of the token before this chunk (0 before the row)
+    for (int base = 0; base < S; base += 32) {
+        const int s = base + lane;
+        const long long v = s < S ? m_row[s] : 0;
+        long long prev = __shfl_up_sync(0xffffffffu, v, 1);
+        if (lane == 0) prev = carry;
+        if (s < S) {
+            const bool ok = v >= 0 && v <= k && (v == 0 || (s == 0 ? v == 1 : prev != 0 && (v == prev || v == prev + 1)));
+            bad |= !ok;
+            if (v != 0) { ++n; m = max(m, (int)min(v, (long long)k)); }
+        }
+        carry = __shfl_sync(0xffffffffu, v, 31);
+    }
+    bad = __any_sync(0xffffffffu, bad);
+    n = __reduce_add_sync(0xffffffffu, n);
+    m = __reduce_max_sync(0xffffffffu, m);
+    if (bad) {
+        if (err_flag && lane == 0) atomicExch(err_flag, 1);
+        n = 0; m = 0;
+    }
+    int* cu = cu_seqlens + (long long)b * (k + 1);
+    // pass 2: a segment starts where the value changes (and at s == 0); position = s - start of the token's segment
+    int seg = 0;                                             // start of the segment the previous chunk ended in
+    carry = 0;
+    for (int base = 0; base < S; base += 32) {
+        const int s = base + lane;
+        const long long v = (s < S && !bad) ? m_row[s] : 0;
+        long long prev = __shfl_up_sync(0xffffffffu, v, 1);
+        if (lane == 0) prev = carry;
+        const bool start = s < S && (s == 0 || v != prev);
+        int st = start ? s : -1;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {                   // inclusive max-scan of segment starts over the chunk
+            const int o = __shfl_up_sync(0xffffffffu, st, d);
+            if (lane >= d) st = max(st, o);
+        }
+        st = max(st, seg);
+        if (s < S) {
+            position_ids[row0 + s] = s - st;
+            if (start && v != 0) {                           // sample v starts here (the tail's start is written below)
+                cu[v - 1] = (int)(row0 + s);
+                cls_index[(long long)b * k + v - 1] = row0 + s;
+            }
+        }
+        seg = __shfl_sync(0xffffffffu, st, 31);
+        carry = __shfl_sync(0xffffffffu, v, 31);
+    }
+    // absent samples are empty segments at the tail's start; the tail is segment k
+    for (int j = m + 1 + lane; j <= k + 1; j += 32) {
+        cu[j - 1] = (int)(row0 + n);
+        if (j <= k) cls_index[(long long)b * k + j - 1] = -1;
+    }
+    if (b == B - 1 && lane == 0) cu_seqlens[(long long)B * (k + 1)] = (int)((long long)B * S);
 }
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ x, bf16* __restrict__ y, long long n) {
     const long long nv = n / 4;
@@ -823,17 +898,19 @@ extern "C" int dle_bias_gelu_bwd(const void* dy, const void* u, void* du, int64_
 extern "C" int dle_embed_ln_fwd(const int64_t* input_ids, const int64_t* token_type_ids, const void* word, const void* pos,
                                 const void* type, const void* gamma, const void* beta, void* z_out, void* y, float* mean,
                                 float* rstd, int32_t B, int32_t S, int32_t H, int32_t V, int32_t P, int32_t NT, float eps,
-                                float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, int32_t* err_flag, void* stream) {
+                                float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, int32_t* err_flag, void* stream,
+                                const int64_t* position_ids) {
     DLE_CHECK_ARG(input_ids && token_type_ids && word && pos && type && gamma && beta && y && mean && rstd);
     DLE_CHECK_ARG(B > 0 && S > 0 && H % 256 == 0 && H > 0 && H <= 1024 && V > 0 && P >= S && NT > 0);
     DLE_CHECK_ARG(ALIGNED16(word) && ALIGNED16(pos) && ALIGNED16(type) && ALIGNED16(y) && ALIGNED16(z_out) && ALIGNED16(gamma) && ALIGNED16(beta));
-    DLE_CHECK_ARG(dropout_p >= 0.f && dropout_p < 1.f);
+    DLE_CHECK_ARG(dropout_p >= 0.f && dropout_p < 1.f && (reinterpret_cast<uintptr_t>(position_ids) & 7) == 0);
     const uint32_t th = dropout_p > 0.f ? dropout_thresh16(dropout_p) : 0u;
     const float sc = dropout_p > 0.f ? 1.f / (1.f - dropout_p) : 1.f;
     const long long T = (long long)B * S;
     LN_DISPATCH(H, (embed_ln_fwd_kernel<J><<<ln_grid(T), LN_THREADS, 0, S_(stream)>>>(
                     reinterpret_cast<const long long*>(input_ids), reinterpret_cast<const long long*>(token_type_ids), B_(word), B_(pos),
-                    B_(type), B_(gamma), B_(beta), BM_(z_out), BM_(y), mean, rstd, B, S, V, P, NT, eps, th, sc, seed, reinterpret_cast<const unsigned long long*>(seed_dev), dropout_stream, err_flag)));
+                    B_(type), B_(gamma), B_(beta), BM_(z_out), BM_(y), mean, rstd, B, S, V, P, NT, eps, th, sc, seed, reinterpret_cast<const unsigned long long*>(seed_dev), dropout_stream, err_flag,
+                    reinterpret_cast<const long long*>(position_ids))));
     DLE_LAUNCH_CHECK();
     return DLE_OK;
 }
@@ -841,16 +918,18 @@ extern "C" int dle_embed_ln_fwd(const int64_t* input_ids, const int64_t* token_t
 extern "C" int dle_embed_ln_bwd(const void* dy, const void* z, const float* mean, const float* rstd, const void* gamma,
                                 const int64_t* input_ids, const int64_t* token_type_ids, float* dword, float* dpos,
                                 float* dtype_tab, float* part_dgamma, float* part_dbeta, int32_t B, int32_t S, int32_t H,
-                                float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, void* stream) {
+                                float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, void* stream,
+                                const int64_t* position_ids) {
     DLE_CHECK_ARG(dy && z && mean && rstd && gamma && input_ids && token_type_ids && dword && dpos && dtype_tab && part_dgamma && part_dbeta);
     DLE_CHECK_ARG(B > 0 && S > 0 && H % 256 == 0 && H > 0 && H <= 1024 && ALIGNED16(dy) && ALIGNED16(z) && ALIGNED16(dword) && ALIGNED16(dpos) && ALIGNED16(dtype_tab));
+    DLE_CHECK_ARG((reinterpret_cast<uintptr_t>(position_ids) & 7) == 0);
     const uint32_t th = dropout_p > 0.f ? dropout_thresh16(dropout_p) : 0u;
     const float sc = dropout_p > 0.f ? 1.f / (1.f - dropout_p) : 1.f;
     const long long T = (long long)B * S;
     LN_DISPATCH(H, (embed_ln_bwd_kernel<J><<<ln_grid(T), LN_THREADS, 0, S_(stream)>>>(
                     B_(dy), B_(z), mean, rstd, B_(gamma), reinterpret_cast<const long long*>(input_ids),
                     reinterpret_cast<const long long*>(token_type_ids), dword, dpos, dtype_tab, part_dgamma, part_dbeta, B, S, th, sc,
-                    seed, reinterpret_cast<const unsigned long long*>(seed_dev), dropout_stream)));
+                    seed, reinterpret_cast<const unsigned long long*>(seed_dev), dropout_stream, reinterpret_cast<const long long*>(position_ids))));
     DLE_LAUNCH_CHECK();
     return DLE_OK;
 }
@@ -867,6 +946,18 @@ extern "C" int dle_scatter_rows(const void* dy, const int64_t* idx, void* dx, in
     DLE_CHECK_ARG(dy && idx && dx && n_idx >= 0 && H > 0 && H % 8 == 0 && n_rows > 0 && ALIGNED16(dy) && ALIGNED16(dx));
     if (n_idx == 0) return DLE_OK;
     scatter_rows_kernel<<<ew_grid(n_idx * (H / 8), 256), 256, 0, S_(stream)>>>(B_(dy), reinterpret_cast<const long long*>(idx), BM_(dx), n_idx, H, n_rows);
+    DLE_LAUNCH_CHECK();
+    return DLE_OK;
+}
+extern "C" int dle_segment_table(const int64_t* mask, int32_t B, int32_t S, int32_t k, int32_t* cu_seqlens, int64_t* position_ids,
+                                 int64_t* cls_index, int32_t* err_flag, void* stream) {
+    DLE_CHECK_ARG(mask && cu_seqlens && position_ids && cls_index && B > 0 && S > 0 && k > 0);
+    DLE_CHECK_ARG((long long)B * (k + 1) <= 65535 && (long long)B * S <= 0x7fffffffLL);
+    DLE_CHECK_ARG(((reinterpret_cast<uintptr_t>(mask) | reinterpret_cast<uintptr_t>(position_ids) | reinterpret_cast<uintptr_t>(cls_index)) & 7) == 0);
+    DLE_CHECK_ARG((reinterpret_cast<uintptr_t>(cu_seqlens) & 3) == 0 && (reinterpret_cast<uintptr_t>(err_flag) & 3) == 0);
+    segment_table_kernel<<<(B + SEG_WARPS - 1) / SEG_WARPS, SEG_WARPS * 32, 0, S_(stream)>>>(
+        reinterpret_cast<const long long*>(mask), B, S, k, cu_seqlens, reinterpret_cast<long long*>(position_ids),
+        reinterpret_cast<long long*>(cls_index), err_flag);
     DLE_LAUNCH_CHECK();
     return DLE_OK;
 }

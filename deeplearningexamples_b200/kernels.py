@@ -259,11 +259,21 @@ def bias_gelu_bwd(dy, u):
 # ------------------------------------------------------------------------------------------------
 # embeddings / gathers / casts
 # ------------------------------------------------------------------------------------------------
+def _check_positions(position_ids, B, S):
+    if position_ids is not None:
+        _req(position_ids, torch.int64, "position_ids")
+        if tuple(position_ids.shape) != (B, S) or not position_ids.is_contiguous():
+            raise L.DleError(f"position_ids must be a contiguous [{B}, {S}] tensor, got shape {tuple(position_ids.shape)}")
+    return position_ids
+
+
 def embed_ln_fwd(input_ids, token_type_ids, word, pos, typ, gamma, beta, *, eps=1e-12, dropout_p=0.0, seed=0,
-                 dropout_stream=0, err_flag=None, seed_dev=None):
+                 dropout_stream=0, err_flag=None, seed_dev=None, position_ids=None):
+    """position_ids: optional int64 [B, S] (None = arange(S) in every row); a position outside the table sets err_flag."""
     lib = L.load()
     _req(input_ids, torch.int64, "input_ids"); _req(token_type_ids, torch.int64, "token_type_ids"); _req(word, bf16, "word")
     B, S = input_ids.shape
+    _check_positions(position_ids, B, S)
     H = word.shape[1]
     T = B * S
     z = torch.empty((T, H), device=word.device, dtype=bf16)
@@ -272,14 +282,16 @@ def embed_ln_fwd(input_ids, token_type_ids, word, pos, typ, gamma, beta, *, eps=
     rstd = torch.empty(T, device=word.device, dtype=torch.float32)
     L.launch_count["n"] += 1; L.check(lib.dle_embed_ln_fwd(_ptr(input_ids), _ptr(token_type_ids), _ptr(word), _ptr(pos), _ptr(typ), _ptr(gamma), _ptr(beta),
                                  _ptr(z), _ptr(y), _ptr(mean), _ptr(rstd), B, S, H, word.shape[0], pos.shape[0], typ.shape[0],
-                                 eps, dropout_p, seed, _ptr(seed_dev), dropout_stream, _ptr(err_flag), _stream()), "dle_embed_ln_fwd")
+                                 eps, dropout_p, seed, _ptr(seed_dev), dropout_stream, _ptr(err_flag), _stream(), _ptr(position_ids)), "dle_embed_ln_fwd")
     return y, z, mean, rstd
 
 
-def embed_ln_bwd(dy, z, mean, rstd, gamma, input_ids, token_type_ids, V, P, NT, *, dropout_p=0.0, seed=0, dropout_stream=0, seed_dev=None):
-    """returns fp32 dword [V,H], dpos [P,H], dtype [NT,H], dgamma [H], dbeta [H]."""
+def embed_ln_bwd(dy, z, mean, rstd, gamma, input_ids, token_type_ids, V, P, NT, *, dropout_p=0.0, seed=0, dropout_stream=0, seed_dev=None,
+                 position_ids=None):
+    """returns fp32 dword [V,H], dpos [P,H], dtype [NT,H], dgamma [H], dbeta [H].  position_ids: those the forward was given."""
     lib = L.load()
     B, S = input_ids.shape
+    _check_positions(position_ids, B, S)
     T, H = dy.shape
     dword = torch.zeros((V, H), device=dy.device, dtype=torch.float32)
     dpos = torch.zeros((P, H), device=dy.device, dtype=torch.float32)
@@ -288,11 +300,28 @@ def embed_ln_bwd(dy, z, mean, rstd, gamma, input_ids, token_type_ids, V, P, NT, 
     parts = torch.empty((2, n_part, H), device=dy.device, dtype=torch.float32)
     L.launch_count["n"] += 1; L.check(lib.dle_embed_ln_bwd(_ptr(dy), _ptr(z), _ptr(mean), _ptr(rstd), _ptr(gamma), _ptr(input_ids), _ptr(token_type_ids),
                                  _ptr(dword), _ptr(dpos), _ptr(dtyp), _ptr(parts[0]), _ptr(parts[1]), B, S, H, dropout_p, seed,
-                                 _ptr(seed_dev), dropout_stream, _stream()), "dle_embed_ln_bwd")
+                                 _ptr(seed_dev), dropout_stream, _stream(), _ptr(position_ids)), "dle_embed_ln_bwd")
     red = torch.empty((2, H), device=dy.device, dtype=torch.float32)
     L.launch_count["n"] += 1; L.check(lib.dle_colsum_finalize_batched(_ptr(parts), 2, n_part, H, _ptr(red), L.DLE_DTYPE_F32, 0, _stream()),
                                       "dle_colsum_finalize_batched")
     return dword, dpos, dtyp, red[0], red[1]
+
+
+def segment_table(mask, k, err_flag=None):
+    """Segment table of a packed batch (include/dle_b200.h, dle_segment_table): mask int64 [B, S] holds each token's sample number
+    (1..k, contiguous and increasing, 0 on the padding tail).  Returns cu_seqlens int32 [B*(k+1) + 1], position_ids int64 [B, S] and
+    cls_index int64 [B*k]; a malformed row sets err_flag and becomes one tail segment."""
+    lib = L.load()
+    _req(mask, torch.int64, "mask")
+    if mask.dim() != 2 or not mask.is_contiguous():
+        raise L.DleError(f"mask must be a contiguous [B, S] tensor, got shape {tuple(mask.shape)}")
+    B, S = mask.shape
+    cu = torch.empty(B * (k + 1) + 1, device=mask.device, dtype=torch.int32)
+    pos = torch.empty((B, S), device=mask.device, dtype=torch.int64)
+    cls = torch.empty(B * k, device=mask.device, dtype=torch.int64)
+    L.launch_count["n"] += 1; L.check(lib.dle_segment_table(_ptr(mask), B, S, k, _ptr(cu), _ptr(pos), _ptr(cls), _ptr(err_flag), _stream()),
+                                      "dle_segment_table")
+    return cu, pos, cls
 
 
 def gather_rows(x, idx, err_flag=None):

@@ -30,6 +30,7 @@ from torch.nn.parameter import Parameter
 from torch.utils import checkpoint
 
 from . import _lib as L
+from . import kernels as K
 from . import ops
 
 bf16 = torch.bfloat16
@@ -203,13 +204,15 @@ class BertEmbeddings(nn.Module):
             self.distill_config = {'use_embedding_states': False}
         self._stream_id = ops.new_stream_id()
 
-    def forward(self, input_ids, token_type_ids):
+    def forward(self, input_ids, token_type_ids, position_ids=None):
+        """position_ids: optional int64 [B, S] on the device (packed samples restart at 0); None reads arange(S) in every row, as the
+        reference does (modeling.py:285-301)."""
         _require_cuda(input_ids, "input_ids")
         B, S = input_ids.shape
         p = self.dropout.p if self.training else 0.0
         y = ops.EmbeddingLNFn.apply(input_ids, token_type_ids, self.word_embeddings.weight, self.position_embeddings.weight,
                                     self.token_type_embeddings.weight, self.LayerNorm.weight, self.LayerNorm.bias,
-                                    p, self.LayerNorm.eps, self._stream_id)
+                                    p, self.LayerNorm.eps, self._stream_id, position_ids)
         embeddings = y.view(B, S, -1)
         if self.distillation and self.distill_config["use_embedding_states"]:
             self.distill_state_dict["embedding_states"] = embeddings
@@ -602,6 +605,20 @@ class BertPreTrainedModel(nn.Module):
                 module._remove_padding_training = bool(val) and bool(training)
         self.apply(_apply_flag)
 
+    def pack_sequences(self, max_per_row):
+        """Sequence packing (off by default; 0 or None turns it off): with it on, every row of a batch holds up to `max_per_row` samples
+        and BertModel.forward reads attention_mask as sample numbers (1..k for the row's k-th sample, 0 on the padding tail; packing.py
+        builds such batches).  Each sample attends to itself only, restarts its position ids and gets its own pooler / NSP row, so
+        the pooled output is [B * max_per_row, H].  Shapes stay static: the route is CUDA-graph capturable.  See BertModel.forward."""
+        k = int(max_per_row or 0)
+        if k < 0:
+            raise L.DleError(f"pack_sequences: max_per_row must be >= 1 (0 or None turns packing off), got {max_per_row}")
+
+        def _apply_flag(module):
+            if hasattr(module, "_pack_per_row"):
+                module._pack_per_row = k
+        self.apply(_apply_flag)
+
     def enable_apex(self, val):
         def _apply_flag(module):
             if hasattr(module, "apex_enabled"):
@@ -693,6 +710,7 @@ class BertModel(BertPreTrainedModel):
         self.teacher = False
         self._remove_padding = False
         self._remove_padding_training = False
+        self._pack_per_row = 0
 
     def forward(self, input_ids, token_type_ids, attention_mask):
         """With remove_padding(True), an inference call (eval mode, grad disabled; anything else raises) whose attention_mask holds
@@ -709,11 +727,22 @@ class BertModel(BertPreTrainedModel):
         row scatter back.  The attention dropout of a right-padded row draws the padded path's keep bits; the dropout of the GEMM
         epilogues and LayerNorms is keyed by packed position instead.  Masked positions get zero rows and zero gradients, so the
         pretraining loss is the padded path's whenever every MLM label lies on a kept position and every row keeps position 0.
-        Activation checkpointing is not supported on the route."""
+        Activation checkpointing is not supported on the route.
+
+        With pack_sequences(k), attention_mask [B, S] holds sample numbers: the tokens of a row's j-th sample hold j (1 <= j <= k),
+        samples are contiguous and increasing, and the padding tail holds 0 and comes last.  One kernel (dle_segment_table) turns it
+        into variable-length sequences on the device, B*(k+1) of them: the k sample slots of each row (empty when absent) and the row's
+        tail, so that every token lies in exactly one sequence.  Embeddings take per-sample position ids, every layer runs
+        BertLayer.forward_packed on the [B*S, H] grid itself (no gather), and the pooler reads each sample's first token ([CLS]):
+        pooled_output is [B*k, H], with tanh(bias) for empty slots.  Values at tail positions are finite but unspecified, as at the
+        padded path's masked positions: no consumer may read them.  A malformed row sets ops.err_flag (raised by
+        ops.check_device_errors()) and runs as one tail segment.  No host read: the route is CUDA-graph capturable."""
         if attention_mask is None:
             attention_mask = torch.ones_like(input_ids)
         if token_type_ids is None:
             token_type_ids = torch.zeros_like(input_ids)
+        if self._pack_per_row:
+            return self._forward_sequence_packed(input_ids, token_type_ids, attention_mask)
         packed = self._pack(attention_mask) if self._remove_padding else None
         if packed is not None:
             encoded_layers = self._encode_packed(input_ids, token_type_ids, *packed)
@@ -778,6 +807,43 @@ class BertModel(BertPreTrainedModel):
             encoded_layers.append(ops.ScatterRowsFn.apply(x, idx, B * S).view(B, S, H))
         return encoded_layers
 
+    def _forward_sequence_packed(self, input_ids, token_type_ids, attention_mask):
+        """BertModel.forward with pack_sequences(k): (encoded_layers, pooled_output [B*k, H])."""
+        k = self._pack_per_row
+        B, S = input_ids.shape
+        if self._remove_padding:
+            raise L.DleError("pack_sequences and remove_padding are two different routes: turn one of them off")
+        if self.encoder._checkpoint_activations:
+            raise L.DleError("pack_sequences does not support activation checkpointing")
+        if not all(layer._fusable() for layer in self.encoder.layer) or not hasattr(self, "pooler"):
+            raise L.DleError("pack_sequences needs the fused layer (head size 64, gelu with bias, no distillation) and the pooler")
+        if S > 512 or S > self.config.max_position_embeddings:
+            raise L.DleError(f"pack_sequences takes S <= 512 and S <= max_position_embeddings, got S = {S}")
+        if B * (k + 1) > 65535:
+            raise L.DleError(f"pack_sequences: B * (max_per_row + 1) = {B * (k + 1)} sequences exceed 65535")
+        _require_cuda(input_ids, "input_ids")
+        _require_cuda(attention_mask, "attention_mask")
+        if self.training:
+            ops.advance_step(input_ids.device)      # as on the padded path: one bump per training forward
+        mask = attention_mask if attention_mask.dtype == torch.int64 else attention_mask.to(torch.int64)
+        cu_seqlens, position_ids, cls_index = K.segment_table(mask.contiguous(), k, err_flag=ops.err_flag(input_ids.device))
+        emb = self.embeddings(input_ids, token_type_ids, position_ids)
+        H = emb.shape[-1]
+        x = emb.view(B * S, H)
+        drop_stride = (S + 63) // 64 * 64           # attention dropout keyed as on a [B*(k+1), S] grid of sequences
+        encoded_layers = []
+        for layer in self.encoder.layer:
+            x = layer.forward_packed(x, cu_seqlens, S, drop_stride)
+            if self.output_all_encoded_layers:
+                encoded_layers.append(x.view(B, S, H).transpose(0, 1))        # (seq, bsz, hidden) views, as BertEncoder returns them
+        if not self.output_all_encoded_layers:
+            encoded_layers.append(x.view(B, S, H))
+        pooled_output = self.pooler.dense_act(ops.GatherRowsFn.apply(x, cls_index))
+        if not self.output_all_encoded_layers:
+            encoded_layers = encoded_layers[-1:]
+        if not self.teacher:
+            return encoded_layers, pooled_output
+
     def make_teacher(self):
         self.teacher = True
 
@@ -811,7 +877,15 @@ class BertForQuestionAnswering(BertPreTrainedModel):
         self.qa_outputs = nn.Linear(config.hidden_size, 2)
         self.apply(self.init_bert_weights)
 
+    def pack_sequences(self, max_per_row):
+        """Refused: a span softmax across a row that holds several samples has no meaning."""
+        if max_per_row:
+            raise L.DleError("pack_sequences is not supported for BertForQuestionAnswering (a span would cross samples)")
+        super().pack_sequences(max_per_row)
+
     def forward(self, input_ids, token_type_ids, attention_mask):
+        if self.bert._pack_per_row:
+            raise L.DleError("pack_sequences is not supported for BertForQuestionAnswering (a span would cross samples)")
         encoded_layers, _ = self.bert(input_ids, token_type_ids, attention_mask)
         sequence_output = encoded_layers[-1]
         logits = self.qa_outputs(sequence_output.to(self.qa_outputs.weight.dtype))

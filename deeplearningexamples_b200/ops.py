@@ -396,30 +396,31 @@ def bert_layer_packed_fwd(x, cu_seqlens, max_seqlen, A, eps, wq, bq, wo, bo, g1,
 
 # -------------------------------------------------------------------------------------------------
 # embeddings: dropout(LayerNorm(word[ids] + pos[arange(S)] + type[tt]))
-# replaces BertEmbeddings.forward (modeling.py:285-301)
+# replaces BertEmbeddings.forward (modeling.py:285-301); position_ids (int64 [B, S], packed samples) replace arange(S) when given
 # -------------------------------------------------------------------------------------------------
 class EmbeddingLNFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, input_ids, token_type_ids, word, pos, typ, gamma, beta, p_drop, eps, stream_id):
+    def forward(ctx, input_ids, token_type_ids, word, pos, typ, gamma, beta, p_drop, eps, stream_id, position_ids=None):
         seed = next_seed() if p_drop > 0.0 else 0
         ids, tts = input_ids.contiguous(), token_type_ids.contiguous()
         y, z, mean, rstd = K.embed_ln_fwd(ids, tts, w16(word), w16(pos), w16(typ), w16(gamma), w16(beta), eps=eps,
                                           dropout_p=p_drop, seed=seed, dropout_stream=stream_id, err_flag=err_flag(word.device),
-                                          seed_dev=step_counter(word.device))
-        ctx.save_for_backward(ids, tts, word, pos, typ, gamma, beta, z, mean, rstd)
+                                          seed_dev=step_counter(word.device), position_ids=position_ids)
+        ctx.save_for_backward(ids, tts, word, pos, typ, gamma, beta, z, mean, rstd, position_ids)
         ctx.cfg = (p_drop, seed, stream_id)
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        ids, tts, word, pos, typ, gamma, beta, z, mean, rstd = ctx.saved_tensors
+        ids, tts, word, pos, typ, gamma, beta, z, mean, rstd, position_ids = ctx.saved_tensors
         p_drop, seed, stream_id = ctx.cfg
         dword, dpos, dtyp, dgamma, dbeta = K.embed_ln_bwd(dy.contiguous(), z, mean, rstd, w16(gamma), ids, tts,
                                                           word.shape[0], pos.shape[0], typ.shape[0], dropout_p=p_drop,
-                                                          seed=seed, dropout_stream=stream_id, seed_dev=step_counter(dy.device))
+                                                          seed=seed, dropout_stream=stream_id, seed_dev=step_counter(dy.device),
+                                                          position_ids=position_ids)
         cast = lambda g, p: g if p.dtype == torch.float32 else K.cast_f32_to_bf16(g)
         return (None, None, cast(dword, word), cast(dpos, pos), cast(dtyp, typ), _to_param_dtype(dgamma, gamma),
-                _to_param_dtype(dbeta, beta), None, None, None)
+                _to_param_dtype(dbeta, beta), None, None, None, None)
 
 
 # -------------------------------------------------------------------------------------------------

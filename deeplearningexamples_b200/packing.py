@@ -1,0 +1,181 @@
+"""Sequence packing on the host: several pretraining samples per S-token row (BertPreTrainedModel.pack_sequences).
+
+The packed batch format (the one BertModel.forward reads in packed mode; dle_segment_table is its device-side reader):
+
+  * input_ids, token_type_ids, labels: int64 [B, S].  Each sample keeps its own [CLS], token types and MLM labels (-1 = none).
+  * attention_mask: int64 [B, S], the sample number of each token: the tokens of a row's j-th sample hold j (1 <= j <= k), samples are
+    contiguous and in increasing order, and the row's padding tail holds 0 and comes last.  k = max_per_row is a static setting.
+  * next_sentence_labels: int64 [B, k], -1 in slots that hold no sample.
+
+Shapes are those of an unpacked batch (plus k NSP slots per row), so a packed step keeps the padded step's static shapes and can be
+captured into a CUDA graph.  The packer places each sample whole (first-fit decreasing over a pool of samples), so a row holds at most
+S tokens, at most k samples and at most `max_pred` MLM labels: the static bound of B * max_pred masked rows holds as for unpacked rows.
+"""
+import numpy as np
+import torch
+
+KEYS = ("input_ids", "token_type_ids", "attention_mask", "labels", "next_sentence_labels")
+
+
+class Sample:
+    """One pretraining sample: ids, token types and MLM labels of its real tokens (1-D int64 numpy arrays) and its NSP label."""
+    __slots__ = ("input_ids", "token_type_ids", "labels", "next_sentence_label", "n_labels")
+
+    def __init__(self, input_ids, token_type_ids, labels, next_sentence_label):
+        self.input_ids, self.token_type_ids, self.labels = input_ids, token_type_ids, labels
+        self.next_sentence_label = int(next_sentence_label)
+        self.n_labels = int((labels != -1).sum())
+
+    def __len__(self):
+        return len(self.input_ids)
+
+
+class PackedBatch(dict):
+    """A packed batch: the five tensors as dict items, and `num_samples`, the number of samples it holds (a host int)."""
+
+    def __init__(self, tensors, num_samples):
+        super().__init__(tensors)
+        self.num_samples = int(num_samples)
+
+
+def split_samples(batch, max_pred=None):
+    """The samples of an unpacked lddl-format batch (0/1 attention_mask, next_sentence_labels [B]): the tokens whose mask is 1, in
+    order, one sample per row; a row without such a token holds no sample.  Raises ValueError for a sample with more than `max_pred`
+    MLM labels, which no packed row could take."""
+    ids, tt, am, lab, nsl = (batch[k].cpu().numpy() for k in KEYS)
+    if am.min(initial=0) < 0 or am.max(initial=0) > 1:
+        raise ValueError("split_samples takes an unpacked batch: attention_mask must hold only 0 and 1")
+    out = []
+    for b in range(ids.shape[0]):
+        keep = am[b] != 0
+        if not keep.any():
+            continue
+        s = Sample(ids[b][keep], tt[b][keep], lab[b][keep], nsl[b])
+        if max_pred is not None and s.n_labels > max_pred:
+            raise ValueError(f"a sample holds {s.n_labels} MLM labels, more than max_predictions_per_seq = {max_pred}")
+        out.append(s)
+    return out
+
+
+def pack(samples, B, S, k, max_pred):
+    """First-fit decreasing: (rows, unplaced).  rows: at most B lists of sample indices, each row within S tokens, k samples and
+    max_pred labels; a row's samples in the order they were placed.  unplaced: the indices that found no room, in increasing order.
+    Ties in length go to the earlier sample, so the result is a function of the list alone."""
+    order = sorted(range(len(samples)), key=lambda i: (-len(samples[i]), i))
+    rows, used = [], []                                  # used[r] = [tokens, samples, labels]
+    unplaced = []
+    for i in order:
+        n, nl = len(samples[i]), samples[i].n_labels
+        if n > S or nl > max_pred:
+            raise ValueError(f"a sample of {n} tokens and {nl} labels does not fit a row of {S} tokens and {max_pred} labels")
+        for r, u in enumerate(used):
+            if u[0] + n <= S and u[1] < k and u[2] + nl <= max_pred:
+                rows[r].append(i)
+                u[0] += n; u[1] += 1; u[2] += nl
+                break
+        else:
+            if len(rows) < B:
+                rows.append([i])
+                used.append([n, 1, nl])
+            else:
+                unplaced.append(i)
+    return rows, sorted(unplaced)
+
+
+def to_batch(samples, rows, B, S, k, pin=False):
+    """The packed batch (PackedBatch of CPU int64 tensors) with rows[r] in row r; rows past len(rows) hold no sample."""
+    ids = np.zeros((B, S), np.int64)
+    tt = np.zeros((B, S), np.int64)
+    am = np.zeros((B, S), np.int64)
+    lab = np.full((B, S), -1, np.int64)
+    nsl = np.full((B, k), -1, np.int64)
+    count = 0
+    for r, members in enumerate(rows):
+        off = 0
+        for j, i in enumerate(members, 1):
+            s = samples[i]
+            n = len(s)
+            ids[r, off:off + n] = s.input_ids
+            tt[r, off:off + n] = s.token_type_ids
+            lab[r, off:off + n] = s.labels
+            am[r, off:off + n] = j
+            nsl[r, j - 1] = s.next_sentence_label
+            off += n
+            count += 1
+    t = {key: torch.from_numpy(v) for key, v in zip(KEYS, (ids, tt, am, lab, nsl))}
+    if pin:
+        t = {key: v.pin_memory() for key, v in t.items()}
+    return PackedBatch(t, count)
+
+
+def unpack(batch):
+    """The samples of a packed batch, row by row and in sample order (the inverse of to_batch)."""
+    ids, tt, am, lab, nsl = (batch[key].cpu().numpy() for key in KEYS)
+    out = []
+    for r in range(ids.shape[0]):
+        for j in range(1, nsl.shape[1] + 1):
+            sel = am[r] == j
+            if sel.any():
+                out.append(Sample(ids[r][sel], tt[r][sel], lab[r][sel], nsl[r, j - 1]))
+    return out
+
+
+def token_fill(batch):
+    """Share of the batch's B*S token slots that hold a sample token."""
+    am = batch["attention_mask"]
+    return float((am != 0).sum()) / am.numel()
+
+
+class PackedLoader:
+    """Packs the batches of any loader of unpacked lddl-format batches (five int64 tensors, 0/1 attention_mask) into PackedBatches of
+    exactly `batch_size` rows.  Samples are drawn into a pool until it holds `pool_rows` * batch_size * seq_len tokens (or the source
+    ends), packed first-fit decreasing, and what finds no room carries over to the next batch.  When the source ends the pool is
+    packed out, so the last batches may hold rows without samples.  Deterministic for a deterministic source."""
+
+    def __init__(self, source, batch_size, seq_len, max_per_row, max_pred, pool_rows=2, pin=False):
+        if max_per_row < 1:
+            raise ValueError(f"max_per_row must be >= 1, got {max_per_row}")
+        self.source, self.B, self.S, self.k, self.P = source, batch_size, seq_len, max_per_row, max_pred
+        self.pool_tokens, self.pin = pool_rows * batch_size * seq_len, pin
+
+    def __iter__(self):
+        pool, it, done = [], iter(self.source), False
+        while True:
+            tokens = sum(len(s) for s in pool)
+            while not done and tokens < self.pool_tokens:
+                try:
+                    new = split_samples(next(it), self.P)
+                except StopIteration:
+                    done = True
+                    break
+                pool += new
+                tokens += sum(len(s) for s in new)
+            if not pool:
+                return
+            rows, unplaced = pack(pool, self.B, self.S, self.k, self.P)
+            yield to_batch(pool, rows, self.B, self.S, self.k, self.pin)
+            pool = [pool[i] for i in unplaced]
+
+
+def synthetic_varlen_batch(B, S, vocab, max_pred, seed=42, round_to=1, mlm_fraction=0.15, pin=False):
+    """An unpacked lddl-format batch of right-padded samples: lengths ~ U{S/4..S} rounded up to `round_to` (capped at S), [CLS] first,
+    token type 1 on the second half of each sample, MLM labels on round(mlm_fraction * length) real tokens after [CLS] (at least one,
+    at most max_pred), random NSP labels."""
+    g = torch.Generator().manual_seed(seed)
+    lens = ((torch.randint(S // 4, S + 1, (B,), generator=g) + round_to - 1) // round_to * round_to).clamp(max=S)
+    ids = torch.randint(0, min(vocab, 30522), (B, S), generator=g, dtype=torch.int64)
+    ids[:, 0] = 101
+    pos = torch.arange(S).unsqueeze(0)
+    am = (pos < lens.unsqueeze(1)).to(torch.int64)
+    tt = ((pos >= (lens // 2).unsqueeze(1)) & (am != 0)).to(torch.int64)
+    labels = torch.full((B, S), -1, dtype=torch.int64)
+    for b in range(B):
+        n = int(lens[b])
+        n_lab = min(max_pred, max(1, round(mlm_fraction * n)), n - 1)
+        where = 1 + torch.randperm(n - 1, generator=g)[:n_lab]
+        labels[b, where] = torch.randint(0, min(vocab, 30522), (n_lab,), generator=g)
+    nsl = torch.randint(0, 2, (B,), generator=g, dtype=torch.int64)
+    batch = {"input_ids": ids, "token_type_ids": tt, "attention_mask": am, "labels": labels, "next_sentence_labels": nsl}
+    if pin:
+        batch = {k: v.pin_memory() for k, v in batch.items()}
+    return batch

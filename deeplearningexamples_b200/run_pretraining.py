@@ -16,6 +16,10 @@ What is different, and why:
   * `--remove_padding` (not in the reference) trains padding-free: every encoder layer runs on the real tokens of the batch only
     (BertModel.remove_padding(True, training=True)).  It reads each batch's mask on the host, so it excludes `--cuda_graphs`, and it
     excludes `--checkpoint_activations`.
+  * `--pack_sequences K` (not in the reference) packs up to K samples into each row (packing.PackedLoader over the loader, and
+    BertPreTrainedModel.pack_sequences(K)).  Shapes stay static, so it works with `--cuda_graphs`, gradient accumulation and DDP; it
+    excludes `--remove_padding` and `--checkpoint_activations`.  With `--input_dir synthetic` the samples have variable lengths.
+    `training_sequences_per_second` still counts rows; `training_samples_per_second` counts the samples of the timed steps.
 """
 import argparse
 import json
@@ -29,7 +33,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from . import modeling, ops
+from . import modeling, ops, packing
 from .lamb import FusedLAMBAMP
 from .schedulers import PolyWarmUpScheduler
 from .training import BertPretrainingCriterion, capture_step_graph, synthetic_batch
@@ -73,8 +77,11 @@ class SyntheticPretrainLoader:
     """`lddl.torch.get_bert_pretrain_data_loader` stand-in: an iterable of pinned batches in the lddl format
     (input_ids, token_type_ids, attention_mask, labels, next_sentence_labels; int64; labels == -1 ignored), sharded by rank."""
 
-    def __init__(self, batch_size, seq_len, max_pred, vocab, steps_per_epoch, base_seed, rank, n_distinct=8):
-        self.batches = [synthetic_batch(batch_size, seq_len, vocab, max_pred, seed=base_seed + rank + 1000 * i, pin=torch.cuda.is_available())
+    def __init__(self, batch_size, seq_len, max_pred, vocab, steps_per_epoch, base_seed, rank, n_distinct=8, variable_length=False):
+        """variable_length: right-padded samples of U{S/4..S} tokens with MLM labels on ~15 % of them (packing.synthetic_varlen_batch)
+        instead of full rows."""
+        make = packing.synthetic_varlen_batch if variable_length else synthetic_batch
+        self.batches = [make(batch_size, seq_len, vocab, max_pred, seed=base_seed + rank + 1000 * i, pin=torch.cuda.is_available())
                         for i in range(n_distinct)]
         self.steps_per_epoch = steps_per_epoch
 
@@ -132,10 +139,17 @@ def parse_arguments(argv=None):
     p.add_argument("--cuda_graphs", default=False, action="store_true")
     p.add_argument("--remove_padding", default=False, action="store_true",
                    help="padding-free training: run the encoder on the real tokens of each batch only (BertModel.remove_padding)")
+    p.add_argument("--pack_sequences", type=int, default=0, metavar="K",
+                   help="pack up to K samples into each row (sequence packing, BertPreTrainedModel.pack_sequences); 0 = off")
     args = p.parse_args(argv)
     if args.remove_padding and (args.cuda_graphs or args.checkpoint_activations):
         raise ValueError("--remove_padding reads each batch's attention mask on the host: it cannot be combined with --cuda_graphs, "
                          "and the padding-free encoder does not support --checkpoint_activations")
+    if args.pack_sequences < 0:
+        raise ValueError("--pack_sequences takes K >= 1 samples per row (0 = off)")
+    if args.pack_sequences and (args.remove_padding or args.checkpoint_activations):
+        raise ValueError("--pack_sequences cannot be combined with --remove_padding (another route), and packed rows do not support "
+                         "--checkpoint_activations")
     args.fp16 = args.fp16 or args.amp
     args.local_rank = int(args.local_rank)
     if args.steps_this_run < 0:
@@ -216,6 +230,8 @@ def prepare_model_and_optimizer(args, device, sequence_output_is_dense):
     model.checkpoint_activations(args.checkpoint_activations)
     if args.remove_padding:
         model.remove_padding(True, training=True)
+    if args.pack_sequences:
+        model.pack_sequences(args.pack_sequences)
     if args.resume_from_checkpoint:
         if (args.phase2 and not args.resume_phase2) or args.init_checkpoint:
             for group in checkpoint['optimizer']['param_groups']:       # new phase: restart the schedule
@@ -333,7 +349,11 @@ def main(argv=None):
     if loader is None:
         steps_needed = int(args.steps_this_run * args.gradient_accumulation_steps) + 64
         loader = SyntheticPretrainLoader(args.train_batch_size, args.max_seq_length, args.max_predictions_per_seq, config.vocab_size,
-                                         steps_needed, args.seed, dist.get_rank() if dist.is_initialized() else 0)
+                                         steps_needed, args.seed, dist.get_rank() if dist.is_initialized() else 0,
+                                         variable_length=bool(args.pack_sequences))
+    if args.pack_sequences:
+        loader = packing.PackedLoader(loader, args.train_batch_size, args.max_seq_length, args.pack_sequences, args.max_predictions_per_seq,
+                                      pin=True)
     logger.log("PARAMETER", {"SEED": args.seed, "train_start": True, "batch_size_per_gpu": args.train_batch_size,
                              "learning_rate": args.learning_rate})
     model.train()
@@ -342,6 +362,7 @@ def main(argv=None):
     skipped_acc = torch.zeros(1, dtype=torch.float32, device=device)
     host = {k: torch.zeros(1, dtype=torch.float32).pin_memory() for k in ("loss", "lr", "skipped")}
     model_step, raw_train_start = 0, None
+    timed_samples = 0               # samples of the timed steps, counted on the host (a packed batch reports its count)
     skip_for_perf = 50 if args.phase2 else 4
     static_batch = full_graph = accum_graph = None
     if args.cuda_graphs:
@@ -360,6 +381,8 @@ def main(argv=None):
             if raw_train_start is None and step == skip_for_perf:
                 torch.cuda.synchronize()
                 raw_train_start = time.time()
+            if raw_train_start is not None:
+                timed_samples += getattr(batch, "num_samples", args.train_batch_size)
             if args.cuda_graphs:
                 for k in batch.keys():
                     static_batch[k].copy_(batch[k], non_blocking=True)
@@ -392,6 +415,10 @@ def main(argv=None):
                             loss_acc.div_(get_world_size())
                             dist.all_reduce(loss_acc)
                         final_loss = loss_acc.item()
+                        samples = torch.tensor([float(timed_samples)], device=device)
+                        if dist.is_initialized():
+                            dist.all_reduce(samples)
+                        args.timed_samples = samples.item()
                         ops.check_device_errors()
                         (model.module if hasattr(model, "module") else model).cls.check_mlm_overflow()
                         logger.log((epoch, dynamic_step), {"final_loss": final_loss})
@@ -411,7 +438,8 @@ def cli(argv=None):
     args, train_time_raw, model_step, skip, final_loss, logger = main(argv)
     if is_main_process():
         perf = args.train_batch_size * get_world_size() * max(model_step - skip, 0) / max(train_time_raw, 1e-9)
-        logger.log((), {"e2e_train_time": time.time() - t0, "training_sequences_per_second": perf, "final_loss": final_loss,
+        logger.log((), {"e2e_train_time": time.time() - t0, "training_sequences_per_second": perf,
+                        "training_samples_per_second": args.timed_samples / max(train_time_raw, 1e-9), "final_loss": final_loss,
                         "raw_train_time": train_time_raw})
     logger.flush()
     if dist.is_initialized():

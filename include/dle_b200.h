@@ -178,15 +178,34 @@ int dle_bias_gelu_bwd(const void* dy, const void* u, void* du, int64_t T, int32_
  *   device flag, may be NULL) instead of faulting.
  * bwd: dz = dLN(dropout_bwd(dy)); scatter-add dz rows into fp32 gradient tables
  *   (dword [V,H], dpos [P,H], dtype [2,H]) with red.global.add; dgamma/dbeta partials as above.
+ * position_ids: int64 [B*S] or NULL.  NULL reads position s = row % S (modeling.py:285-301 builds arange(S) per row); otherwise
+ *   the position of token row r is position_ids[r] (packed samples restart at 0).  Dropout stays keyed by element index, so
+ *   position_ids = arange(S) per row gives the NULL path's bits.  The forward treats a position outside [0, P) like an out-of-range
+ *   id (sets *err_flag, reads row 0); the backward takes the forward's ids and positions as they are.
  * ------------------------------------------------------------------------------------------ */
 int dle_embed_ln_fwd(const int64_t* input_ids, const int64_t* token_type_ids, const void* word, const void* pos,
                      const void* type, const void* gamma, const void* beta, void* z_out, void* y, float* mean,
                      float* rstd, int32_t B, int32_t S, int32_t H, int32_t V, int32_t P, int32_t NT, float eps,
-                     float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, int32_t* err_flag, void* stream);
+                     float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, int32_t* err_flag, void* stream,
+                     const int64_t* position_ids);
 int dle_embed_ln_bwd(const void* dy, const void* z, const float* mean, const float* rstd, const void* gamma,
                      const int64_t* input_ids, const int64_t* token_type_ids, float* dword, float* dpos,
                      float* dtype_tab, float* part_dgamma, float* part_dbeta, int32_t B, int32_t S, int32_t H,
-                     float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, void* stream);
+                     float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, void* stream,
+                     const int64_t* position_ids);
+/* segment table of a packed batch (several samples per row; replaces the position ids of modeling.py:285-301 and the [CLS] row the
+ * pooler reads at modeling.py:518-523).  mask: int64 [B, S], the sample number of each token: the j-th sample of a row (1 <= j <= k)
+ * holds j, samples are contiguous and increasing, and the row's padding tail holds 0 and comes last.  Outputs, all static in size:
+ *   cu_seqlens   int32 [B*(k+1) + 1]: row b owns sequences b*(k+1) .. b*(k+1)+k; sequence b*(k+1)+j-1 is sample j (length 0 when the
+ *                row has fewer than j samples) and b*(k+1)+k is the row's padding tail.  A row's lengths sum to S, so every token lies in
+ *                exactly one sequence and row b starts at b*S.
+ *   position_ids int64 [B*S]: index of the token inside its sample (inside the tail for tail tokens).
+ *   cls_index    int64 [B*k]: b*S + start of sample j at b*k + j-1, or -1 when the row has no sample j (dle_gather_rows: a zero row).
+ * A malformed row (a value outside 0..k, a decrease, a skipped number, a non-zero value after a 0) sets *err_flag (may be NULL) and is
+ * written as one tail segment of length S with positions 0..S-1 and no samples.  One warp per row, no host work: graph-capturable.
+ * B*(k+1) <= 65535. */
+int dle_segment_table(const int64_t* mask, int32_t B, int32_t S, int32_t k, int32_t* cu_seqlens, int64_t* position_ids,
+                      int64_t* cls_index, int32_t* err_flag, void* stream);
 /* masked-row gather (dense sequence output): out[i,:] = x[idx[i],:]  -- bit exact.
  * replaces torch.index_select at modeling.py:590.  bwd scatters rows back (rows are unique).
  * idx[i] == -1 marks a PADDING slot of a static-size index list (torch.nonzero_static): gather writes a zero row, scatter skips it;
