@@ -769,6 +769,52 @@ segment_table_kernel(const long long* __restrict__ mask, int B, int S, int k, in
     }
     if (b == B - 1 && lane == 0) cu_seqlens[(long long)B * (k + 1)] = (int)((long long)B * S);
 }
+// ---------------------------------------------------------------------------------------------
+// per-sample span logits of a packed batch: the QA head's [B*S, 2] output on the packed grid <-> [B*k, S] start / end rows,
+// one per sample slot; slot b*k + j is sequence b*(k+1) + j of the segment table.  Pure moves: bit exact both ways.
+// ---------------------------------------------------------------------------------------------
+template <typename T>
+__global__ void span_logits_unpack_kernel(const T* __restrict__ logits, long long ld, const int* __restrict__ cu_seqlens, int S, int k,
+                                          long long n, float fill, T* __restrict__ start_out, T* __restrict__ end_out) {
+    const T f = static_cast<T>(fill);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const long long slot = i / S;
+        const int p = (int)(i - slot * S);
+        const long long seq = slot / k * (k + 1) + slot % k;
+        const int c0 = cu_seqlens[seq];
+        T s = f, e = f;
+        if (p < cu_seqlens[seq + 1] - c0) {
+            const T* row = logits + (long long)(c0 + p) * ld;
+            s = row[0];
+            e = row[1];
+        }
+        start_out[i] = s;
+        end_out[i] = e;
+    }
+}
+// one thread per grid token: every row of dlogits is written exactly once (tail tokens get 0), so no memset and no atomics
+template <typename T>
+__global__ void span_logits_pack_grad_kernel(const T* __restrict__ dstart, const T* __restrict__ dend, const int* __restrict__ cu_seqlens,
+                                             int S, int k, long long n, T* __restrict__ dlogits, long long ld) {
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < n; t += (long long)gridDim.x * blockDim.x) {
+        const long long b = t / S;
+        const int* cu = cu_seqlens + b * (k + 1);
+        // the row's sequence holding t: the last of its k+1 starts that is <= t (an empty slot starts where the next one does)
+        int lo = 0, hi = k;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (cu[mid] <= t) lo = mid; else hi = mid - 1;
+        }
+        T ds = static_cast<T>(0.f), de = static_cast<T>(0.f);
+        if (lo < k) {                                          // lo == k: the row's padding tail
+            const long long o = (b * k + lo) * S + (t - cu[lo]);
+            ds = dstart[o];
+            de = dend[o];
+        }
+        dlogits[t * ld] = ds;
+        dlogits[t * ld + 1] = de;
+    }
+}
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ x, bf16* __restrict__ y, long long n) {
     const long long nv = n / 4;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += (long long)gridDim.x * blockDim.x) {
@@ -958,6 +1004,43 @@ extern "C" int dle_segment_table(const int64_t* mask, int32_t B, int32_t S, int3
     segment_table_kernel<<<(B + SEG_WARPS - 1) / SEG_WARPS, SEG_WARPS * 32, 0, S_(stream)>>>(
         reinterpret_cast<const long long*>(mask), B, S, k, cu_seqlens, reinterpret_cast<long long*>(position_ids),
         reinterpret_cast<long long*>(cls_index), err_flag);
+    DLE_LAUNCH_CHECK();
+    return DLE_OK;
+}
+static bool span_logits_args_ok(const void* a, const void* b, const void* c, const int32_t* cu_seqlens, int32_t B, int32_t S, int32_t k,
+                                int32_t dtype, int64_t ld) {
+    if (!(a && b && c && cu_seqlens && B > 0 && S > 0 && k > 0 && ld >= 2)) return false;
+    if ((long long)B * (k + 1) > 65535 || (long long)B * S > 0x7fffffffLL) return false;
+    if (dtype != DLE_DTYPE_F32 && dtype != DLE_DTYPE_BF16) return false;
+    const uintptr_t align = dtype == DLE_DTYPE_F32 ? 3 : 1;
+    return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & align) == 0 &&
+           (reinterpret_cast<uintptr_t>(cu_seqlens) & 3) == 0;
+}
+extern "C" int dle_span_logits_unpack(const void* logits, int64_t ld, const int32_t* cu_seqlens, int32_t B, int32_t S, int32_t k,
+                                      int32_t dtype, float fill, void* start_out, void* end_out, void* stream) {
+    DLE_CHECK_ARG(span_logits_args_ok(logits, start_out, end_out, cu_seqlens, B, S, k, dtype, ld));
+    const long long n = (long long)B * k * S;
+    if (dtype == DLE_DTYPE_F32)
+        span_logits_unpack_kernel<float><<<ew_grid(n, 256), 256, 0, S_(stream)>>>(
+            reinterpret_cast<const float*>(logits), ld, cu_seqlens, S, k, n, fill, reinterpret_cast<float*>(start_out),
+            reinterpret_cast<float*>(end_out));
+    else
+        span_logits_unpack_kernel<bf16><<<ew_grid(n, 256), 256, 0, S_(stream)>>>(B_(logits), ld, cu_seqlens, S, k, n, fill,
+                                                                                  BM_(start_out), BM_(end_out));
+    DLE_LAUNCH_CHECK();
+    return DLE_OK;
+}
+extern "C" int dle_span_logits_pack_grad(const void* dstart, const void* dend, const int32_t* cu_seqlens, int32_t B, int32_t S, int32_t k,
+                                         int32_t dtype, void* dlogits, int64_t ld, void* stream) {
+    DLE_CHECK_ARG(span_logits_args_ok(dstart, dend, dlogits, cu_seqlens, B, S, k, dtype, ld));
+    const long long n = (long long)B * S;
+    if (dtype == DLE_DTYPE_F32)
+        span_logits_pack_grad_kernel<float><<<ew_grid(n, 256), 256, 0, S_(stream)>>>(
+            reinterpret_cast<const float*>(dstart), reinterpret_cast<const float*>(dend), cu_seqlens, S, k, n,
+            reinterpret_cast<float*>(dlogits), ld);
+    else
+        span_logits_pack_grad_kernel<bf16><<<ew_grid(n, 256), 256, 0, S_(stream)>>>(B_(dstart), B_(dend), cu_seqlens, S, k, n,
+                                                                                     BM_(dlogits), ld);
     DLE_LAUNCH_CHECK();
     return DLE_OK;
 }

@@ -324,6 +324,50 @@ def segment_table(mask, k, err_flag=None):
     return cu, pos, cls
 
 
+_DTYPE_CODE = {torch.float32: L.DLE_DTYPE_F32, bf16: L.DLE_DTYPE_BF16}
+
+
+def _span_dtype(t, name):
+    _req(t, name=name)
+    if t.dtype not in _DTYPE_CODE:
+        raise L.DleError(f"{name} must be bfloat16 or float32, got {t.dtype}")
+    return _DTYPE_CODE[t.dtype]
+
+
+def span_logits_unpack(logits, cu_seqlens, B, S, k, fill=-10000.0):
+    """Per-sample span logits of a packed batch (include/dle_b200.h, dle_span_logits_unpack): logits [B*S, 2] (bf16 or fp32, last dim
+    contiguous) and cu_seqlens of segment_table(mask, k) -> (start, end), each [B*k, S] of the logits' dtype, left-aligned per sample
+    and `fill` everywhere else."""
+    lib = L.load()
+    code = _span_dtype(logits, "logits")
+    _req(cu_seqlens, torch.int32, "cu_seqlens")
+    if tuple(logits.shape) != (B * S, 2) or cu_seqlens.numel() != B * (k + 1) + 1 or not cu_seqlens.is_contiguous():
+        raise L.DleError(f"span_logits_unpack: logits must be [{B * S}, 2] and cu_seqlens [{B * (k + 1) + 1}], got "
+                         f"{tuple(logits.shape)} and {tuple(cu_seqlens.shape)}")
+    ld = _row_major_2d(logits, "logits")
+    start = torch.empty((B * k, S), device=logits.device, dtype=logits.dtype)
+    end = torch.empty_like(start)
+    L.launch_count["n"] += 1; L.check(lib.dle_span_logits_unpack(_ptr(logits), ld, _ptr(cu_seqlens), B, S, k, code, fill, _ptr(start), _ptr(end),
+                                                                 _stream()), "dle_span_logits_unpack")
+    return start, end
+
+
+def span_logits_pack_grad(dstart, dend, cu_seqlens, B, S, k):
+    """The gradient of span_logits_unpack: dstart, dend [B*k, S] -> dlogits [B*S, 2] of their dtype (0 at every tail token)."""
+    lib = L.load()
+    code = _span_dtype(dstart, "dstart")
+    _req(dend, dstart.dtype, "dend"); _req(cu_seqlens, torch.int32, "cu_seqlens")
+    for t, name in ((dstart, "dstart"), (dend, "dend")):
+        if tuple(t.shape) != (B * k, S) or not t.is_contiguous():
+            raise L.DleError(f"{name} must be a contiguous [{B * k}, {S}] tensor, got shape {tuple(t.shape)}")
+    if cu_seqlens.numel() != B * (k + 1) + 1 or not cu_seqlens.is_contiguous():
+        raise L.DleError(f"cu_seqlens must hold {B * (k + 1) + 1} entries, got {tuple(cu_seqlens.shape)}")
+    dlogits = torch.empty((B * S, 2), device=dstart.device, dtype=dstart.dtype)
+    L.launch_count["n"] += 1; L.check(lib.dle_span_logits_pack_grad(_ptr(dstart), _ptr(dend), _ptr(cu_seqlens), B, S, k, code, _ptr(dlogits), 2,
+                                                                    _stream()), "dle_span_logits_pack_grad")
+    return dlogits
+
+
 def gather_rows(x, idx, err_flag=None):
     lib = L.load()
     _req(x, bf16, "x"); _req(idx, torch.int64, "idx")

@@ -809,14 +809,26 @@ class BertModel(BertPreTrainedModel):
 
     def _forward_sequence_packed(self, input_ids, token_type_ids, attention_mask):
         """BertModel.forward with pack_sequences(k): (encoded_layers, pooled_output [B*k, H])."""
+        if not hasattr(self, "pooler"):
+            raise L.DleError("pack_sequences needs the pooler")
+        encoded_layers, x, _, cls_index = self._encode_sequence_packed(input_ids, token_type_ids, attention_mask)
+        pooled_output = self.pooler.dense_act(ops.GatherRowsFn.apply(x, cls_index))
+        if not self.output_all_encoded_layers:
+            encoded_layers = encoded_layers[-1:]
+        if not self.teacher:
+            return encoded_layers, pooled_output
+
+    def _encode_sequence_packed(self, input_ids, token_type_ids, attention_mask):
+        """Embeddings and encoder of the pack_sequences(k) route: (encoded_layers, last layer's output [B*S, H], cu_seqlens,
+        cls_index), the last two from the one dle_segment_table launch of the forward."""
         k = self._pack_per_row
         B, S = input_ids.shape
         if self._remove_padding:
             raise L.DleError("pack_sequences and remove_padding are two different routes: turn one of them off")
         if self.encoder._checkpoint_activations:
             raise L.DleError("pack_sequences does not support activation checkpointing")
-        if not all(layer._fusable() for layer in self.encoder.layer) or not hasattr(self, "pooler"):
-            raise L.DleError("pack_sequences needs the fused layer (head size 64, gelu with bias, no distillation) and the pooler")
+        if not all(layer._fusable() for layer in self.encoder.layer):
+            raise L.DleError("pack_sequences needs the fused layer (head size 64, gelu with bias, no distillation)")
         if S > 512 or S > self.config.max_position_embeddings:
             raise L.DleError(f"pack_sequences takes S <= 512 and S <= max_position_embeddings, got S = {S}")
         if B * (k + 1) > 65535:
@@ -838,11 +850,7 @@ class BertModel(BertPreTrainedModel):
                 encoded_layers.append(x.view(B, S, H).transpose(0, 1))        # (seq, bsz, hidden) views, as BertEncoder returns them
         if not self.output_all_encoded_layers:
             encoded_layers.append(x.view(B, S, H))
-        pooled_output = self.pooler.dense_act(ops.GatherRowsFn.apply(x, cls_index))
-        if not self.output_all_encoded_layers:
-            encoded_layers = encoded_layers[-1:]
-        if not self.teacher:
-            return encoded_layers, pooled_output
+        return encoded_layers, x, cu_seqlens, cls_index
 
     def make_teacher(self):
         self.teacher = True
@@ -876,18 +884,44 @@ class BertForQuestionAnswering(BertPreTrainedModel):
         self.bert = BertModel(config)
         self.qa_outputs = nn.Linear(config.hidden_size, 2)
         self.apply(self.init_bert_weights)
+        self._per_sample_logits = False
 
-    def pack_sequences(self, max_per_row):
-        """Refused: a span softmax across a row that holds several samples has no meaning."""
-        if max_per_row:
-            raise L.DleError("pack_sequences is not supported for BertForQuestionAnswering (a span would cross samples)")
+    # logits outside a packed sample: the reference's mask constant (modeling.py:864-872); exact 0 in a real sample's fp32 softmax,
+    # and finite, so the log-softmax backward of an ignored empty slot stays finite too
+    SPAN_FILL = -10000.0
+
+    def pack_sequences(self, max_per_row, per_sample_logits=False):
+        """Sequence packing for SQuAD fine-tuning (off by default; 0 or None turns it off).  A span softmax across a row that holds
+        several samples has no meaning, so packing needs per_sample_logits=True: forward then reads attention_mask as sample numbers
+        (packing.py, the SQuAD format) and returns start_logits and end_logits of shape [B*max_per_row, S].  Slot b*k + j-1 holds
+        sample j of row b, left-aligned: entry p is the sample's own token p, as in an unpacked feature, and every other entry is
+        SPAN_FILL (an empty slot is SPAN_FILL throughout).  Shapes stay static: the route is CUDA-graph capturable."""
+        if max_per_row and not per_sample_logits:
+            raise L.DleError("pack_sequences on BertForQuestionAnswering needs per_sample_logits=True (a span would cross samples)")
         super().pack_sequences(max_per_row)
+        self._per_sample_logits = bool(self.bert._pack_per_row)
 
     def forward(self, input_ids, token_type_ids, attention_mask):
-        if self.bert._pack_per_row:
-            raise L.DleError("pack_sequences is not supported for BertForQuestionAnswering (a span would cross samples)")
+        k = self.bert._pack_per_row
+        if k:
+            if not self._per_sample_logits:
+                raise L.DleError("BertForQuestionAnswering packs sequences only through its own pack_sequences(k, "
+                                 "per_sample_logits=True) (a span would cross samples)")
+            return self._forward_packed_spans(input_ids, token_type_ids, attention_mask, k)
         encoded_layers, _ = self.bert(input_ids, token_type_ids, attention_mask)
         sequence_output = encoded_layers[-1]
         logits = self.qa_outputs(sequence_output.to(self.qa_outputs.weight.dtype))
         start_logits, end_logits = logits.split(1, dim=-1)
         return start_logits.squeeze(-1), end_logits.squeeze(-1)
+
+    def _forward_packed_spans(self, input_ids, token_type_ids, attention_mask, k):
+        """The packed encoder (no pooler: the QA model never reads it), the QA head on the [B, S, H] grid exactly as the padded forward
+        calls it, and one kernel that moves each sample's logits into its own slot row."""
+        if attention_mask is None:
+            attention_mask = torch.ones_like(input_ids)
+        if token_type_ids is None:
+            token_type_ids = torch.zeros_like(input_ids)
+        B, S = input_ids.shape
+        _, x, cu_seqlens, _ = self.bert._encode_sequence_packed(input_ids, token_type_ids, attention_mask)
+        logits = self.qa_outputs(x.view(B, S, -1).to(self.qa_outputs.weight.dtype))
+        return ops.SpanLogitsUnpackFn.apply(logits.view(B * S, 2), cu_seqlens, B, S, k, self.SPAN_FILL)

@@ -468,6 +468,26 @@ class ScatterRowsFn(torch.autograd.Function):
 
 
 # -------------------------------------------------------------------------------------------------
+# per-sample span logits of a packed SQuAD batch: the QA head's [B*S, 2] logits -> start / end [B*k, S], one row per sample slot,
+# `fill` outside the sample (modeling.py:1366-1369 and the span loss of run_squad.py:1066-1079, one feature per row)
+# -------------------------------------------------------------------------------------------------
+class SpanLogitsUnpackFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logits, cu_seqlens, B, S, k, fill):
+        ctx.save_for_backward(cu_seqlens)
+        ctx.shape = (B, S, k)
+        return K.span_logits_unpack(logits, cu_seqlens, B, S, k, fill)
+
+    @staticmethod
+    def backward(ctx, dstart, dend):
+        (cu_seqlens,) = ctx.saved_tensors
+        B, S, k = ctx.shape
+        dstart = torch.zeros_like(dend) if dstart is None else dstart.contiguous()
+        dend = torch.zeros_like(dstart) if dend is None else dend.contiguous()
+        return K.span_logits_pack_grad(dstart, dend, cu_seqlens, B, S, k), None, None, None, None, None
+
+
+# -------------------------------------------------------------------------------------------------
 # mean cross-entropy over the vocabulary on bf16 logits, fp32 arithmetic, no fp32 copy of the logits
 # replaces CrossEntropyLoss(ignore_index=-1) on the MLM scores (run_pretraining.py:85-95)
 # -------------------------------------------------------------------------------------------------

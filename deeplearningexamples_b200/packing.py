@@ -10,6 +10,16 @@ The packed batch format (the one BertModel.forward reads in packed mode; dle_seg
 Shapes are those of an unpacked batch (plus k NSP slots per row), so a packed step keeps the padded step's static shapes and can be
 captured into a CUDA graph.  The packer places each sample whole (first-fit decreasing over a pool of samples), so a row holds at most
 S tokens, at most k samples and at most `max_pred` MLM labels: the static bound of B * max_pred masked rows holds as for unpacked rows.
+
+The packed SQuAD format (BertForQuestionAnswering.pack_sequences(k, per_sample_logits=True); the keys squad.squad_training_step
+reads):
+
+  * input_ids, segment_ids: int64 [B, S].  Each feature keeps its own [CLS] question [SEP] context [SEP] tokens and segment ids.
+  * input_mask: int64 [B, S], sample numbers 1..k and 0 on the tail, exactly as attention_mask above.
+  * start_positions, end_positions: int64 [B*k].  Slot b*k + j-1 holds sample j of row b; a position counts from the sample's first
+    token.  An empty slot, and an answer outside the feature, hold S: the loss's ignore_index (run_squad.py:1073-1079).
+  * feature_index (a host attribute of the PackedBatch, numpy int64 [B*k]): the index of the SQuAD feature in each slot, -1 when the
+    slot is empty.  Evaluation maps the [B*k, S] logits back to their features through it.
 """
 import numpy as np
 import torch
@@ -30,8 +40,24 @@ class Sample:
         return len(self.input_ids)
 
 
+class SquadSample:
+    """One SQuAD feature: ids and segment ids of its real tokens (1-D int64 numpy arrays), its answer's start and end relative to its
+    first token (S or more: no answer in this feature, ignored by the loss) and the index of the feature in its source stream."""
+    __slots__ = ("input_ids", "segment_ids", "start_position", "end_position", "feature_index")
+    n_labels = 0                                         # no MLM labels: pack()'s label bound never binds
+
+    def __init__(self, input_ids, segment_ids, start_position, end_position, feature_index):
+        self.input_ids, self.segment_ids = input_ids, segment_ids
+        self.start_position, self.end_position = int(start_position), int(end_position)
+        self.feature_index = int(feature_index)
+
+    def __len__(self):
+        return len(self.input_ids)
+
+
 class PackedBatch(dict):
-    """A packed batch: the five tensors as dict items, and `num_samples`, the number of samples it holds (a host int)."""
+    """A packed batch: the five tensors as dict items, and `num_samples`, the number of samples it holds (a host int).  A SQuAD batch
+    also carries `feature_index` (see the module docstring)."""
 
     def __init__(self, tensors, num_samples):
         super().__init__(tensors)
@@ -120,9 +146,74 @@ def unpack(batch):
     return out
 
 
+SQUAD_KEYS = ("input_ids", "segment_ids", "input_mask", "start_positions", "end_positions")
+
+
+def split_squad_samples(batch, first_feature_index=0):
+    """The features of an unpacked SQuAD batch (0/1 input_mask, right-padded rows, start/end_positions [B]): the tokens whose mask is
+    1, one feature per row, feature index first_feature_index + row; a row without such a token holds no feature."""
+    ids, seg, am, sp, ep = (batch[key].cpu().numpy() for key in SQUAD_KEYS)
+    if am.min(initial=0) < 0 or am.max(initial=0) > 1:
+        raise ValueError("split_squad_samples takes an unpacked batch: input_mask must hold only 0 and 1")
+    out = []
+    for b in range(ids.shape[0]):
+        keep = am[b] != 0
+        if keep.any():
+            out.append(SquadSample(ids[b][keep], seg[b][keep], sp[b], ep[b], first_feature_index + b))
+    return out
+
+
+def to_squad_batch(samples, rows, B, S, k, pin=False):
+    """The packed SQuAD batch (PackedBatch of CPU int64 tensors, with feature_index) with rows[r] in row r.  A position of S or more
+    becomes S (ignored, as the reference's clamp makes it); a position inside [len, S) points into a padded row's padding, which a
+    packed sample does not have: ValueError."""
+    ids = np.zeros((B, S), np.int64)
+    seg = np.zeros((B, S), np.int64)
+    am = np.zeros((B, S), np.int64)
+    pos = np.full((2, B * k), S, np.int64)
+    fi = np.full(B * k, -1, np.int64)
+    count = 0
+    for r, members in enumerate(rows):
+        off = 0
+        for j, i in enumerate(members, 1):
+            s = samples[i]
+            n = len(s)
+            for c, p in enumerate((s.start_position, s.end_position)):
+                if n <= p < S:
+                    raise ValueError(f"feature {s.feature_index}: answer position {p} lies in the padding of its row (length {n}, "
+                                     f"S = {S}); only positions < {n} or >= {S} (ignored) have a meaning per sample")
+                pos[c, r * k + j - 1] = min(p, S)
+            ids[r, off:off + n] = s.input_ids
+            seg[r, off:off + n] = s.segment_ids
+            am[r, off:off + n] = j
+            fi[r * k + j - 1] = s.feature_index
+            off += n
+            count += 1
+    t = {key: torch.from_numpy(v) for key, v in zip(SQUAD_KEYS, (ids, seg, am, pos[0], pos[1]))}
+    if pin:
+        t = {key: v.pin_memory() for key, v in t.items()}
+    batch = PackedBatch(t, count)
+    batch.feature_index = fi
+    return batch
+
+
+def unpack_squad(batch):
+    """The features of a packed SQuAD batch in slot order (the inverse of to_squad_batch, with positions past the sample as S)."""
+    ids, seg, am, sp, ep = (batch[key].cpu().numpy() for key in SQUAD_KEYS)
+    k = sp.shape[0] // ids.shape[0]
+    out = []
+    for r in range(ids.shape[0]):
+        for j in range(1, k + 1):
+            sel = am[r] == j
+            if sel.any():
+                slot = r * k + j - 1
+                out.append(SquadSample(ids[r][sel], seg[r][sel], sp[slot], ep[slot], batch.feature_index[slot]))
+    return out
+
+
 def token_fill(batch):
     """Share of the batch's B*S token slots that hold a sample token."""
-    am = batch["attention_mask"]
+    am = batch["input_mask"] if "input_mask" in batch else batch["attention_mask"]
     return float((am != 0).sum()) / am.numel()
 
 
@@ -130,30 +221,39 @@ class PackedLoader:
     """Packs the batches of any loader of unpacked lddl-format batches (five int64 tensors, 0/1 attention_mask) into PackedBatches of
     exactly `batch_size` rows.  Samples are drawn into a pool until it holds `pool_rows` * batch_size * seq_len tokens (or the source
     ends), packed first-fit decreasing, and what finds no room carries over to the next batch.  When the source ends the pool is
-    packed out, so the last batches may hold rows without samples.  Deterministic for a deterministic source."""
+    packed out, so the last batches may hold rows without samples.  Deterministic for a deterministic source.
 
-    def __init__(self, source, batch_size, seq_len, max_per_row, max_pred, pool_rows=2, pin=False):
+    squad=True packs unpacked SQuAD batches (SQUAD_KEYS, 0/1 input_mask) into the packed SQuAD format instead; max_pred is unused
+    then, and feature indices count the source's rows from 0."""
+
+    def __init__(self, source, batch_size, seq_len, max_per_row, max_pred=0, pool_rows=2, pin=False, squad=False):
         if max_per_row < 1:
             raise ValueError(f"max_per_row must be >= 1, got {max_per_row}")
         self.source, self.B, self.S, self.k, self.P = source, batch_size, seq_len, max_per_row, max_pred
-        self.pool_tokens, self.pin = pool_rows * batch_size * seq_len, pin
+        self.pool_tokens, self.pin, self.squad = pool_rows * batch_size * seq_len, pin, squad
 
     def __iter__(self):
         pool, it, done = [], iter(self.source), False
+        rows_seen = 0
         while True:
             tokens = sum(len(s) for s in pool)
             while not done and tokens < self.pool_tokens:
                 try:
-                    new = split_samples(next(it), self.P)
+                    batch = next(it)
                 except StopIteration:
                     done = True
                     break
+                if self.squad:
+                    new = split_squad_samples(batch, rows_seen)
+                    rows_seen += batch["input_ids"].shape[0]
+                else:
+                    new = split_samples(batch, self.P)
                 pool += new
                 tokens += sum(len(s) for s in new)
             if not pool:
                 return
             rows, unplaced = pack(pool, self.B, self.S, self.k, self.P)
-            yield to_batch(pool, rows, self.B, self.S, self.k, self.pin)
+            yield (to_squad_batch if self.squad else to_batch)(pool, rows, self.B, self.S, self.k, self.pin)
             pool = [pool[i] for i in unplaced]
 
 

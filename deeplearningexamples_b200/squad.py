@@ -9,6 +9,13 @@ the reference step's structure (PyTorch/LanguageModeling/BERT/run_squad.py):
 
 Differences: bf16 instead of fp16 (no loss scaling needed; a GradScaler can still be passed), the clip is part of the optimizer
 launch instead of a separate l2norm + scale sweep, the schedule can live on the device (CUDA-graph capturable).
+
+Packed features: with model.pack_sequences(k, per_sample_logits=True), squad_training_step and training.capture_step_graph take a
+packed SQuAD batch (packing.py: input_mask holds sample numbers, start/end_positions are [B*k], one per sample slot, S in an empty
+slot) unchanged.  The logits are [B*k, S], each sample's own positions first and BertForQuestionAnswering.SPAN_FILL after them, so
+squad_loss clamps to [0, S] and ignores S exactly as on padded rows.  A sample's cross-entropy then runs over its own len positions:
+it equals the padded route's on the same feature with the logits of its padding positions set to SPAN_FILL (the padded route also
+softmaxes over its padding logits).  The mean runs over the counted slots, one term per feature, as the reference's does.
 """
 import torch
 
@@ -43,6 +50,23 @@ def synthetic_squad_batch(B, S, vocab, seed=42, full_mask=True, device="cpu", pi
     if device != "cpu":
         batch = {k: v.to(device) for k, v in batch.items()}
     return batch
+
+
+def synthetic_squad_features(B, S, vocab, seed=42):
+    """Variable-length SQuAD features as an unpacked batch (right-padded rows, 0/1 input_mask) that packing.PackedLoader(squad=True)
+    also takes: lengths ~ U{S/4..S} as synthetic_squad_batch(full_mask=False), [CLS] first, segment 1 on the last three quarters of
+    each feature, and an answer span inside it (start ~ U{0..len-1}, end ~ U{start..len-1})."""
+    g = torch.Generator().manual_seed(seed)
+    lens = torch.randint(S // 4, S + 1, (B,), generator=g)
+    ids = torch.randint(0, min(vocab, 30522), (B, S), generator=g, dtype=torch.int64)
+    ids[:, 0] = 101
+    pos = torch.arange(S).unsqueeze(0)
+    am = (pos < lens.unsqueeze(1)).to(torch.int64)
+    ids *= am
+    seg = ((pos >= (lens // 4).unsqueeze(1)) & (am != 0)).to(torch.int64)
+    start = (torch.rand(B, generator=g) * lens).long()
+    end = start + (torch.rand(B, generator=g) * (lens - start)).long()
+    return {"input_ids": ids, "input_mask": am, "segment_ids": seg, "start_positions": start, "end_positions": end}
 
 
 def prepare_squad_model_and_optimizer(config_dict, device, *, learning_rate=3e-5, warmup_proportion=0.1, total_steps=1000,

@@ -206,6 +206,20 @@ int dle_embed_ln_bwd(const void* dy, const void* z, const float* mean, const flo
  * B*(k+1) <= 65535. */
 int dle_segment_table(const int64_t* mask, int32_t B, int32_t S, int32_t k, int32_t* cu_seqlens, int64_t* position_ids,
                       int64_t* cls_index, int32_t* err_flag, void* stream);
+/* per-sample span logits of a packed SQuAD batch (several features per row; serves the split of the QA head's logits at
+ * modeling.py:1366-1369 and the span cross-entropy over them at run_squad.py:1066-1079, which must see one feature per row).
+ *   unpack:    logits [B*S, 2] with row stride ld (column 0 start, column 1 end) on the packed grid, and cu_seqlens of
+ *              dle_segment_table for the same B, S, k.  Slot b*k + j-1 holds sample j of row b (sequence b*(k+1) + j-1):
+ *              start_out[b*k + j-1, p] = logits[cu + p, 0] for p < len, and fill for len <= p < S and across an empty slot;
+ *              end_out likewise from column 1.  start_out, end_out: [B*k, S], contiguous.
+ *   pack_grad: the inverse for the gradients: dlogits[cu + p] = (dstart[slot, p], dend[slot, p]) for every sample token, and exactly
+ *              (0, 0) at every tail token.  Every row of dlogits is written once (no memset needed).
+ * Both only move values: bit exact.  dtype DLE_DTYPE_BF16 or DLE_DTYPE_F32 for every tensor (fill is rounded to it).  No host work:
+ * graph-capturable.  A malformed row is one tail segment in the table, so all its slots come out as fill.  B*(k+1) <= 65535. */
+int dle_span_logits_unpack(const void* logits, int64_t ld, const int32_t* cu_seqlens, int32_t B, int32_t S, int32_t k,
+                           int32_t dtype, float fill, void* start_out, void* end_out, void* stream);
+int dle_span_logits_pack_grad(const void* dstart, const void* dend, const int32_t* cu_seqlens, int32_t B, int32_t S, int32_t k,
+                              int32_t dtype, void* dlogits, int64_t ld, void* stream);
 /* masked-row gather (dense sequence output): out[i,:] = x[idx[i],:]  -- bit exact.
  * replaces torch.index_select at modeling.py:590.  bwd scatters rows back (rows are unique).
  * idx[i] == -1 marks a PADDING slot of a static-size index list (torch.nonzero_static): gather writes a zero row, scatter skips it;
