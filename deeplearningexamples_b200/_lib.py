@@ -63,6 +63,9 @@ SIGNATURES = {
     "dle_segment_table": (_i32, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "dle_span_logits_unpack": (_i32, [_vp, _i64, _vp, _i32, _i32, _i32, _i32, _f32, _vp, _vp, _vp]),
     "dle_span_logits_pack_grad": (_i32, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _i64, _vp]),
+    "dle_cls_head_fwd": (_i32, [_vp, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _f32, _u64, _vp, _u32, _vp, _vp]),
+    "dle_cls_head_bwd_partials": (_i32, [_i32]),
+    "dle_cls_head_bwd": (_i32, [_vp, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _f32, _u64, _vp, _u32, _vp, _vp, _vp, _vp, _vp]),
     "dle_gather_rows": (_i32, [_vp, _vp, _vp, _i64, _i32, _i64, _vp, _vp]),
     "dle_scatter_rows": (_i32, [_vp, _vp, _vp, _i64, _i32, _i64, _vp]),
     "dle_advance_u64": (_i32, [_vp, _u64, _vp]),

@@ -815,6 +815,113 @@ __global__ void span_logits_pack_grad_kernel(const T* __restrict__ dstart, const
         dlogits[t * ld + 1] = de;
     }
 }
+// ---------------------------------------------------------------------------------------------
+// sequence-classification head: logits[r, l] = sum_c dropout(x)[r, c] * W[l, c] + b[l] (modeling.py:1145-1155), L <= 32 labels,
+// too narrow for the GEMM (N % 8).  The dropout keep bit of x[r, c] is that of flat element r*H + c, as at every hidden-dropout site.
+// Each row's arithmetic depends on that row alone.
+// ---------------------------------------------------------------------------------------------
+__device__ __forceinline__ float ld_f32(const float* p) { return *p; }
+__device__ __forceinline__ float ld_f32(const bf16* p) { return __bfloat162float(*p); }
+__device__ __forceinline__ void st_f32(float* p, float v) { *p = v; }
+__device__ __forceinline__ void st_f32(bf16* p, float v) { *p = __float2bfloat16_rn(v); }
+
+// forward: one warp per row, lane owns the 8-column units lane, lane + 32, ...; labels CLS_LC at a time (dropout redrawn per pass);
+// lane-order fp32 partial sums, then a butterfly warp sum: a fixed order per row
+constexpr int CLS_WARPS = 8, CLS_LC = 4;
+template <typename T>
+__global__ void __launch_bounds__(CLS_WARPS * 32)
+cls_head_fwd_kernel(const bf16* __restrict__ x, long long ldx, const bf16* __restrict__ w, const T* __restrict__ b, int R, int H, int L,
+                    uint32_t thresh, float drop_scale, unsigned long long seed, const unsigned long long* seed_dev, uint32_t stream_id,
+                    T* __restrict__ logits) {
+    seed = effective_seed(seed, seed_dev);
+    const int lane = threadIdx.x & 31;
+    const long long r = (long long)blockIdx.x * CLS_WARPS + (threadIdx.x >> 5);
+    if (r >= R) return;
+    const bf16* xr = x + r * ldx;
+    const unsigned long long g0 = (unsigned long long)r * (unsigned)(H >> 5);     // group32 of element r*H + col: g0 + col / 32
+    for (int l0 = 0; l0 < L; l0 += CLS_LC) {
+        float acc[CLS_LC] = {0.f, 0.f, 0.f, 0.f};
+        for (int col = lane * 8; col < H; col += 256) {
+            float xv[8];
+            unpack8(ld_global_nc_v4(xr + col), xv);
+            if (thresh != 0u) {
+                const uint32_t keep = dropout_keep8(seed, stream_id, g0 + (col >> 5), (col & 31) >> 3, thresh);
+#pragma unroll
+                for (int i = 0; i < 8; ++i) xv[i] = ((keep >> i) & 1u) ? xv[i] * drop_scale : 0.f;
+            }
+#pragma unroll
+            for (int j = 0; j < CLS_LC; ++j) {
+                if (l0 + j < L) {
+                    float wv[8];
+                    unpack8(ld_global_nc_v4(w + (long long)(l0 + j) * H + col), wv);
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) acc[j] = fmaf(xv[i], wv[i], acc[j]);
+                }
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < CLS_LC; ++j) {
+            const float s = warp_sum(acc[j]);
+            if (lane == j && l0 + j < L) st_f32(logits + r * L + l0 + j, s + ld_f32(b + l0 + j));
+        }
+    }
+}
+
+// backward: CTA (column block of CLSB_THREADS, slab of CLSB_ROWS rows), one thread per column.  dx is written per element; dW and db
+// go to per-slab fp32 partials (rows in order), which colsum_finalize_kernel sums over slabs in a fixed order: no atomics.
+constexpr int CLSB_THREADS = 256, CLSB_ROWS = 32;
+template <typename T, int LMAX>
+__global__ void __launch_bounds__(CLSB_THREADS)
+cls_head_bwd_kernel(const T* __restrict__ dlogits, const bf16* __restrict__ x, long long ldx, const bf16* __restrict__ w, int R, int H,
+                    int L, uint32_t thresh, float drop_scale, unsigned long long seed, const unsigned long long* seed_dev,
+                    uint32_t stream_id, bf16* __restrict__ dx, float* __restrict__ part_dw, float* __restrict__ part_db) {
+    __shared__ float d_s[CLSB_ROWS][LMAX];
+    seed = effective_seed(seed, seed_dev);
+    const long long r0 = (long long)blockIdx.y * CLSB_ROWS;
+    const int nr = (int)min((long long)CLSB_ROWS, R - r0);
+    for (int i = threadIdx.x; i < CLSB_ROWS * LMAX; i += CLSB_THREADS) {
+        const int rr = i / LMAX, l = i % LMAX;
+        d_s[rr][l] = (rr < nr && l < L) ? ld_f32(dlogits + (r0 + rr) * L + l) : 0.f;
+    }
+    __syncthreads();
+    if (blockIdx.x == 0 && threadIdx.x < L) {
+        float s = 0.f;
+        for (int rr = 0; rr < nr; ++rr) s += d_s[rr][threadIdx.x];
+        part_db[(long long)blockIdx.y * L + threadIdx.x] = s;
+    }
+    const int c = blockIdx.x * CLSB_THREADS + threadIdx.x;
+    if (c >= H) return;
+    float wc[LMAX], acc[LMAX];
+#pragma unroll
+    for (int l = 0; l < LMAX; ++l) {
+        wc[l] = l < L ? __bfloat162float(w[(long long)l * H + c]) : 0.f;
+        acc[l] = 0.f;
+    }
+    for (int rr = 0; rr < nr; ++rr) {
+        const long long r = r0 + rr;
+        const float xv = __bfloat162float(x[r * ldx + c]);
+        bool kept = true;
+        float sc = 1.f;
+        if (thresh != 0u) {
+            kept = (dropout_keep8(seed, stream_id, (unsigned long long)(r * H + c) >> 5, (c & 31) >> 3, thresh) >> (c & 7)) & 1u;
+            sc = drop_scale;
+        }
+        const float xd = kept ? xv * sc : 0.f;
+        float g = 0.f;
+#pragma unroll
+        for (int l = 0; l < LMAX; ++l) {
+            if (l < L) {
+                const float d = d_s[rr][l];
+                g = fmaf(d, wc[l], g);
+                acc[l] = fmaf(d, xd, acc[l]);
+            }
+        }
+        dx[r * H + c] = __float2bfloat16_rn(kept ? g * sc : 0.f);
+    }
+#pragma unroll
+    for (int l = 0; l < LMAX; ++l)
+        if (l < L) part_dw[((long long)blockIdx.y * L + l) * H + c] = acc[l];
+}
 __global__ void cast_f32_bf16_kernel(const float* __restrict__ x, bf16* __restrict__ y, long long n) {
     const long long nv = n / 4;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += (long long)gridDim.x * blockDim.x) {
@@ -1043,6 +1150,56 @@ extern "C" int dle_span_logits_pack_grad(const void* dstart, const void* dend, c
                                                                                      BM_(dlogits), ld);
     DLE_LAUNCH_CHECK();
     return DLE_OK;
+}
+static bool cls_head_args_ok(const void* x, int64_t ldx, const void* w, int32_t R, int32_t H, int32_t L, int32_t dtype, float dropout_p) {
+    if (!(x && w && R > 0 && H > 0 && H % 32 == 0 && L >= 1 && L <= 32 && ldx >= H && ldx % 8 == 0)) return false;
+    if ((long long)R > 65535LL * CLSB_ROWS || (dtype != DLE_DTYPE_F32 && dtype != DLE_DTYPE_BF16)) return false;
+    return dropout_p >= 0.f && dropout_p < 1.f && ALIGNED16(x) && ALIGNED16(w);
+}
+static bool dtype_aligned(const void* p, int32_t dtype) {
+    return (reinterpret_cast<uintptr_t>(p) & (dtype == DLE_DTYPE_F32 ? 3 : 1)) == 0;
+}
+extern "C" int dle_cls_head_fwd(const void* x, int64_t ldx, const void* w, const void* b, int32_t R, int32_t H, int32_t L, int32_t dtype,
+                                float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, void* logits,
+                                void* stream) {
+    DLE_CHECK_ARG(cls_head_args_ok(x, ldx, w, R, H, L, dtype, dropout_p) && b && logits);
+    DLE_CHECK_ARG(dtype_aligned(b, dtype) && dtype_aligned(logits, dtype));
+    const uint32_t th = dropout_p > 0.f ? dropout_thresh16(dropout_p) : 0u;
+    const float sc = dropout_p > 0.f ? 1.f / (1.f - dropout_p) : 1.f;
+    const auto sdev = reinterpret_cast<const unsigned long long*>(seed_dev);
+    const int grid = (R + CLS_WARPS - 1) / CLS_WARPS;
+    if (dtype == DLE_DTYPE_F32)
+        cls_head_fwd_kernel<float><<<grid, CLS_WARPS * 32, 0, S_(stream)>>>(B_(x), ldx, B_(w), reinterpret_cast<const float*>(b), R, H, L,
+                                                                            th, sc, seed, sdev, dropout_stream, reinterpret_cast<float*>(logits));
+    else
+        cls_head_fwd_kernel<bf16><<<grid, CLS_WARPS * 32, 0, S_(stream)>>>(B_(x), ldx, B_(w), B_(b), R, H, L, th, sc, seed, sdev,
+                                                                           dropout_stream, BM_(logits));
+    DLE_LAUNCH_CHECK();
+    return DLE_OK;
+}
+extern "C" int dle_cls_head_bwd_partials(int32_t R) { return R > 0 ? (R + CLSB_ROWS - 1) / CLSB_ROWS : DLE_ERR_INVALID; }
+extern "C" int dle_cls_head_bwd(const void* dlogits, const void* x, int64_t ldx, const void* w, int32_t R, int32_t H, int32_t L,
+                                int32_t dtype, float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, void* dx,
+                                float* part, void* dw, void* db, void* stream) {
+    DLE_CHECK_ARG(cls_head_args_ok(x, ldx, w, R, H, L, dtype, dropout_p) && dlogits && dx && part && dw && db);
+    DLE_CHECK_ARG(dtype_aligned(dlogits, dtype) && dtype_aligned(dw, dtype) && dtype_aligned(db, dtype));
+    DLE_CHECK_ARG((reinterpret_cast<uintptr_t>(dx) & 1) == 0 && (reinterpret_cast<uintptr_t>(part) & 3) == 0);
+    const uint32_t th = dropout_p > 0.f ? dropout_thresh16(dropout_p) : 0u;
+    const float sc = dropout_p > 0.f ? 1.f / (1.f - dropout_p) : 1.f;
+    const auto sdev = reinterpret_cast<const unsigned long long*>(seed_dev);
+    const int n_part = (R + CLSB_ROWS - 1) / CLSB_ROWS;
+    float* part_dw = part;
+    float* part_db = part + (long long)n_part * L * H;
+    const dim3 grid((H + CLSB_THREADS - 1) / CLSB_THREADS, n_part);
+#define CLS_BWD(T, LM, D) cls_head_bwd_kernel<T, LM><<<grid, CLSB_THREADS, 0, S_(stream)>>>(D, B_(x), ldx, B_(w), R, H, L, th, sc, seed, \
+                                                                                         sdev, dropout_stream, BM_(dx), part_dw, part_db)
+    const float* d32 = reinterpret_cast<const float*>(dlogits);
+    if (dtype == DLE_DTYPE_F32) { if (L <= 4) CLS_BWD(float, 4, d32); else CLS_BWD(float, 32, d32); }
+    else { if (L <= 4) CLS_BWD(bf16, 4, B_(dlogits)); else CLS_BWD(bf16, 32, B_(dlogits)); }
+#undef CLS_BWD
+    DLE_LAUNCH_CHECK();
+    if (int rc = dle_colsum_finalize(part_dw, n_part, L * H, dw, dtype, 0, stream)) return rc;
+    return dle_colsum_finalize(part_db, n_part, L, db, dtype, 0, stream);
 }
 __global__ void advance_u64_kernel(unsigned long long* c, unsigned long long d) { *c += d; }
 extern "C" int dle_advance_u64(uint64_t* counter, uint64_t delta, void* stream) {

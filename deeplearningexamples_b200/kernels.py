@@ -368,6 +368,57 @@ def span_logits_pack_grad(dstart, dend, cu_seqlens, B, S, k):
     return dlogits
 
 
+def _cls_head_x(x, w):
+    """x as the head kernels take it (bf16 [R, H], row stride a multiple of 8, 16-byte aligned) and its row stride."""
+    _req(x, bf16, "x"); _req(w, bf16, "w")
+    if x.dim() != 2 or w.dim() != 2 or x.shape[1] != w.shape[1] or not w.is_contiguous():
+        raise L.DleError(f"cls_head: x must be [R, H] and w a contiguous [L, H], got {tuple(x.shape)} and {tuple(w.shape)}")
+    ld = _row_major_2d(x, "x")
+    if ld % 8 or x.data_ptr() % 16:
+        x = x.contiguous()
+        ld = x.shape[1]
+    return x, ld
+
+
+def cls_head_fwd(x, w, b, dropout_p=0.0, seed=0, dropout_stream=0, seed_dev=None):
+    """Sequence-classification head (include/dle_b200.h, dle_cls_head_fwd): x [R, H] bf16, w [L, H] bf16, b [L] bf16 or fp32 ->
+    logits [R, L] of b's dtype, logits = dropout(x) @ w^T + b with the hidden-dropout keep bits of element r*H + c."""
+    lib = L.load()
+    x, ldx = _cls_head_x(x, w)
+    code = _span_dtype(b, "b")
+    R, H = x.shape
+    n_lab = w.shape[0]
+    if tuple(b.shape) != (n_lab,) or not b.is_contiguous():
+        raise L.DleError(f"b must be a contiguous [{n_lab}] tensor, got shape {tuple(b.shape)}")
+    logits = torch.empty((R, n_lab), device=x.device, dtype=b.dtype)
+    L.launch_count["n"] += 1; L.check(lib.dle_cls_head_fwd(_ptr(x), ldx, _ptr(w), _ptr(b), R, H, n_lab, code, dropout_p, seed, _ptr(seed_dev),
+                                                           dropout_stream, _ptr(logits), _stream()), "dle_cls_head_fwd")
+    return logits
+
+
+def cls_head_bwd(dlogits, x, w, dropout_p=0.0, seed=0, dropout_stream=0, seed_dev=None):
+    """The gradients of cls_head_fwd for dlogits [R, L] (bf16 or fp32, the parameter dtype): (dx [R, H] bf16, dw [L, H], db [L]), dw and
+    db of dlogits' dtype, summed over rows in a fixed order.  The dropout arguments must be those of the forward."""
+    lib = L.load()
+    x, ldx = _cls_head_x(x, w)
+    code = _span_dtype(dlogits, "dlogits")
+    R, H = x.shape
+    n_lab = w.shape[0]
+    if tuple(dlogits.shape) != (R, n_lab) or not dlogits.is_contiguous():
+        raise L.DleError(f"dlogits must be a contiguous [{R}, {n_lab}] tensor, got shape {tuple(dlogits.shape)}")
+    n_part = lib.dle_cls_head_bwd_partials(R)
+    if n_part <= 0:
+        raise L.DleError(f"cls_head_bwd: R = {R} rows")
+    part = torch.empty(n_part * n_lab * (H + 1), device=x.device, dtype=torch.float32)
+    dx = torch.empty((R, H), device=x.device, dtype=bf16)
+    dw = torch.empty((n_lab, H), device=x.device, dtype=dlogits.dtype)
+    db = torch.empty((n_lab,), device=x.device, dtype=dlogits.dtype)
+    L.launch_count["n"] += 3; L.check(lib.dle_cls_head_bwd(_ptr(dlogits), _ptr(x), ldx, _ptr(w), R, H, n_lab, code, dropout_p, seed,
+                                                           _ptr(seed_dev), dropout_stream, _ptr(dx), _ptr(part), _ptr(dw), _ptr(db),
+                                                           _stream()), "dle_cls_head_bwd")
+    return dx, dw, db
+
+
 def gather_rows(x, idx, err_flag=None):
     lib = L.load()
     _req(x, bf16, "x"); _req(idx, torch.int64, "idx")

@@ -925,3 +925,39 @@ class BertForQuestionAnswering(BertPreTrainedModel):
         _, x, cu_seqlens, _ = self.bert._encode_sequence_packed(input_ids, token_type_ids, attention_mask)
         logits = self.qa_outputs(x.view(B, S, -1).to(self.qa_outputs.weight.dtype))
         return ops.SpanLogitsUnpackFn.apply(logits.view(B * S, 2), cu_seqlens, B, S, k, self.SPAN_FILL)
+
+
+class BertForSequenceClassification(BertPreTrainedModel):
+    """Sequence-classification head over the pooled output (reference modeling.py:1129-1155): logits = classifier(dropout(pooled)).
+    forward(input_ids, token_type_ids=None, attention_mask=None) -> logits [B, num_labels] in the parameter dtype.
+
+    `dropout` stays an nn.Dropout module (train() / eval() and its `p` behave as in the reference), but the dropout and the classifier
+    run in one kernel each way (ops.ClassifierHeadFn): the mask is drawn from the device step counter like every other hidden-dropout
+    mask, so a captured training step draws a fresh mask on every replay.  With pack_sequences(k), attention_mask holds sample
+    numbers (packing.py, the GLUE format) and the logits are [B*k, num_labels]: slot b*k + j-1 holds sample j of row b, and an empty
+    slot holds the head applied to tanh(pooler bias) -- finite and meaningless, for a label the loss ignores."""
+
+    def __init__(self, config, num_labels):
+        super().__init__(config)
+        self.distillation = getattr(config, 'distillation', False)
+        if self.distillation:
+            self.distill_state_dict = OrderedDict()
+            self.distill_config = config.distillation_config
+        self.num_labels = num_labels
+        self.bert = BertModel(config)
+        if not self.distillation or self.distill_config["use_pred_states"]:
+            self.dropout = nn.Dropout(config.hidden_dropout_prob)
+            self.classifier = nn.Linear(config.hidden_size, num_labels)
+        self.apply(self.init_bert_weights)
+        self._stream_id = ops.new_stream_id()
+
+    def forward(self, input_ids, token_type_ids=None, attention_mask=None):
+        _, pooled_output = self.bert(input_ids, token_type_ids, attention_mask)
+        if not self.distillation or self.distill_config["use_pred_states"]:
+            p = self.dropout.p if self.dropout.training else 0.0
+            x = pooled_output if pooled_output.dtype == bf16 else pooled_output.to(bf16)
+            final_output = ops.ClassifierHeadFn.apply(x, self.classifier.weight, self.classifier.bias, p, self._stream_id)
+            if self.distillation and self.distill_config["use_pred_states"]:
+                self.distill_state_dict["pred_states"] = final_output
+            if not self.distillation or not self.training:
+                return final_output

@@ -488,6 +488,29 @@ class SpanLogitsUnpackFn(torch.autograd.Function):
 
 
 # -------------------------------------------------------------------------------------------------
+# logits = classifier(dropout(pooled)): the sequence-classification head in one kernel each way
+# replaces BertForSequenceClassification's dropout + nn.Linear (modeling.py:1145-1155); masks keyed like every hidden-dropout site
+# -------------------------------------------------------------------------------------------------
+class ClassifierHeadFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, weight, bias, p_drop, stream_id):
+        seed = next_seed() if p_drop > 0.0 else 0
+        logits = K.cls_head_fwd(x, w16(weight), bias.detach(), dropout_p=p_drop, seed=seed, dropout_stream=stream_id,
+                                seed_dev=step_counter(x.device))
+        ctx.save_for_backward(x, weight, bias)
+        ctx.cfg = (p_drop, seed, stream_id)
+        return logits
+
+    @staticmethod
+    def backward(ctx, dlogits):
+        x, weight, bias = ctx.saved_tensors
+        p_drop, seed, stream_id = ctx.cfg
+        dx, dw, db = K.cls_head_bwd(dlogits.to(bias.dtype).contiguous(), x, w16(weight), dropout_p=p_drop, seed=seed,
+                                    dropout_stream=stream_id, seed_dev=step_counter(x.device))
+        return dx, _to_param_dtype(dw, weight), _to_param_dtype(db, bias), None, None
+
+
+# -------------------------------------------------------------------------------------------------
 # mean cross-entropy over the vocabulary on bf16 logits, fp32 arithmetic, no fp32 copy of the logits
 # replaces CrossEntropyLoss(ignore_index=-1) on the MLM scores (run_pretraining.py:85-95)
 # -------------------------------------------------------------------------------------------------

@@ -20,6 +20,15 @@ reads):
     token.  An empty slot, and an answer outside the feature, hold S: the loss's ignore_index (run_squad.py:1073-1079).
   * feature_index (a host attribute of the PackedBatch, numpy int64 [B*k]): the index of the SQuAD feature in each slot, -1 when the
     slot is empty.  Evaluation maps the [B*k, S] logits back to their features through it.
+
+The packed GLUE format (BertForSequenceClassification.pack_sequences(k); the keys glue.glue_training_step reads, run_glue.py's batch):
+
+  * input_ids, segment_ids: int64 [B, S].  Each example keeps its own [CLS] a [SEP] b [SEP] tokens and segment ids.
+  * input_mask: int64 [B, S], sample numbers 1..k and 0 on the tail, exactly as attention_mask above.
+  * label_ids: int64 [B*k].  Slot b*k + j-1 holds sample j of row b; an empty slot holds -100, the default ignore_index of the
+    reference's CrossEntropyLoss (run_glue.py:597), so its loss line runs unchanged and averages over the real samples.
+  * example_index (a host attribute of the PackedBatch, numpy int64 [B*k]): the index of the example in each slot, -1 when the slot
+    is empty.  Evaluation maps the [B*k, num_labels] logits back to their examples through it.
 """
 import numpy as np
 import torch
@@ -55,9 +64,23 @@ class SquadSample:
         return len(self.input_ids)
 
 
+class GlueSample:
+    """One GLUE example: ids and segment ids of its real tokens (1-D int64 numpy arrays), its label and the index of the example in
+    its source stream."""
+    __slots__ = ("input_ids", "segment_ids", "label", "example_index")
+    n_labels = 0                                         # no MLM labels: pack()'s label bound never binds
+
+    def __init__(self, input_ids, segment_ids, label, example_index):
+        self.input_ids, self.segment_ids = input_ids, segment_ids
+        self.label, self.example_index = int(label), int(example_index)
+
+    def __len__(self):
+        return len(self.input_ids)
+
+
 class PackedBatch(dict):
-    """A packed batch: the five tensors as dict items, and `num_samples`, the number of samples it holds (a host int).  A SQuAD batch
-    also carries `feature_index` (see the module docstring)."""
+    """A packed batch: the tensors as dict items, and `num_samples`, the number of samples it holds (a host int).  A SQuAD batch also
+    carries `feature_index`, a GLUE batch `example_index` (see the module docstring)."""
 
     def __init__(self, tensors, num_samples):
         super().__init__(tensors)
@@ -211,6 +234,72 @@ def unpack_squad(batch):
     return out
 
 
+GLUE_KEYS = ("input_ids", "segment_ids", "input_mask", "label_ids")
+GLUE_IGNORE = -100                                       # CrossEntropyLoss's default ignore_index
+
+
+def split_glue_samples(batch, first_example_index=0):
+    """The examples of an unpacked GLUE batch (0/1 input_mask, right-padded rows, label_ids [B]): the tokens whose mask is 1, one
+    example per row, example index first_example_index + row; a row without such a token holds no example."""
+    ids, seg, am, lab = (batch[key].cpu().numpy() for key in GLUE_KEYS)
+    if am.min(initial=0) < 0 or am.max(initial=0) > 1:
+        raise ValueError("split_glue_samples takes an unpacked batch: input_mask must hold only 0 and 1")
+    out = []
+    for b in range(ids.shape[0]):
+        keep = am[b] != 0
+        if keep.any():
+            out.append(GlueSample(ids[b][keep], seg[b][keep], lab[b], first_example_index + b))
+    return out
+
+
+def to_glue_batch(samples, rows, B, S, k, pin=False):
+    """The packed GLUE batch (PackedBatch of CPU int64 tensors, with example_index) with rows[r] in row r; rows past len(rows) and
+    slots past a row's samples are empty (label -100, example index -1).  ValueError when a row exceeds S tokens or k samples."""
+    ids = np.zeros((B, S), np.int64)
+    seg = np.zeros((B, S), np.int64)
+    am = np.zeros((B, S), np.int64)
+    lab = np.full(B * k, GLUE_IGNORE, np.int64)
+    ei = np.full(B * k, -1, np.int64)
+    if len(rows) > B:
+        raise ValueError(f"{len(rows)} rows do not fit a batch of {B}")
+    count = 0
+    for r, members in enumerate(rows):
+        n_row = sum(len(samples[i]) for i in members)
+        if n_row > S or len(members) > k:
+            raise ValueError(f"row {r}: {len(members)} samples of {n_row} tokens do not fit a row of {k} samples and {S} tokens")
+        off = 0
+        for j, i in enumerate(members, 1):
+            s = samples[i]
+            n = len(s)
+            ids[r, off:off + n] = s.input_ids
+            seg[r, off:off + n] = s.segment_ids
+            am[r, off:off + n] = j
+            lab[r * k + j - 1] = s.label
+            ei[r * k + j - 1] = s.example_index
+            off += n
+            count += 1
+    t = {key: torch.from_numpy(v) for key, v in zip(GLUE_KEYS, (ids, seg, am, lab))}
+    if pin:
+        t = {key: v.pin_memory() for key, v in t.items()}
+    batch = PackedBatch(t, count)
+    batch.example_index = ei
+    return batch
+
+
+def unpack_glue(batch):
+    """The examples of a packed GLUE batch in slot order (the inverse of to_glue_batch)."""
+    ids, seg, am, lab = (batch[key].cpu().numpy() for key in GLUE_KEYS)
+    k = lab.shape[0] // ids.shape[0]
+    out = []
+    for r in range(ids.shape[0]):
+        for j in range(1, k + 1):
+            sel = am[r] == j
+            if sel.any():
+                slot = r * k + j - 1
+                out.append(GlueSample(ids[r][sel], seg[r][sel], lab[slot], batch.example_index[slot]))
+    return out
+
+
 def token_fill(batch):
     """Share of the batch's B*S token slots that hold a sample token."""
     am = batch["input_mask"] if "input_mask" in batch else batch["attention_mask"]
@@ -224,13 +313,16 @@ class PackedLoader:
     packed out, so the last batches may hold rows without samples.  Deterministic for a deterministic source.
 
     squad=True packs unpacked SQuAD batches (SQUAD_KEYS, 0/1 input_mask) into the packed SQuAD format instead; max_pred is unused
-    then, and feature indices count the source's rows from 0."""
+    then, and feature indices count the source's rows from 0.  glue=True does the same for unpacked GLUE batches (GLUE_KEYS) and
+    the packed GLUE format, with example indices counting the source's rows from 0."""
 
-    def __init__(self, source, batch_size, seq_len, max_per_row, max_pred=0, pool_rows=2, pin=False, squad=False):
+    def __init__(self, source, batch_size, seq_len, max_per_row, max_pred=0, pool_rows=2, pin=False, squad=False, glue=False):
         if max_per_row < 1:
             raise ValueError(f"max_per_row must be >= 1, got {max_per_row}")
+        if squad and glue:
+            raise ValueError("PackedLoader packs one format: pass squad=True or glue=True, not both")
         self.source, self.B, self.S, self.k, self.P = source, batch_size, seq_len, max_per_row, max_pred
-        self.pool_tokens, self.pin, self.squad = pool_rows * batch_size * seq_len, pin, squad
+        self.pool_tokens, self.pin, self.squad, self.glue = pool_rows * batch_size * seq_len, pin, squad, glue
 
     def __iter__(self):
         pool, it, done = [], iter(self.source), False
@@ -243,8 +335,8 @@ class PackedLoader:
                 except StopIteration:
                     done = True
                     break
-                if self.squad:
-                    new = split_squad_samples(batch, rows_seen)
+                if self.squad or self.glue:
+                    new = (split_squad_samples if self.squad else split_glue_samples)(batch, rows_seen)
                     rows_seen += batch["input_ids"].shape[0]
                 else:
                     new = split_samples(batch, self.P)
@@ -253,7 +345,8 @@ class PackedLoader:
             if not pool:
                 return
             rows, unplaced = pack(pool, self.B, self.S, self.k, self.P)
-            yield (to_squad_batch if self.squad else to_batch)(pool, rows, self.B, self.S, self.k, self.pin)
+            fmt = to_squad_batch if self.squad else to_glue_batch if self.glue else to_batch
+            yield fmt(pool, rows, self.B, self.S, self.k, self.pin)
             pool = [pool[i] for i in unplaced]
 
 

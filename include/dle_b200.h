@@ -220,6 +220,25 @@ int dle_span_logits_unpack(const void* logits, int64_t ld, const int32_t* cu_seq
                            int32_t dtype, float fill, void* start_out, void* end_out, void* stream);
 int dle_span_logits_pack_grad(const void* dstart, const void* dend, const int32_t* cu_seqlens, int32_t B, int32_t S, int32_t k,
                               int32_t dtype, void* dlogits, int64_t ld, void* stream);
+/* sequence-classification head: dropout of the pooled rows, then the [H] -> [L] classifier (modeling.py:1145-1155, the
+ * BertForSequenceClassification forward whose logits run_glue.py:631-634 feeds to CrossEntropyLoss).  L is too narrow for the GEMM.
+ *   fwd: x [R, H] bf16 (row stride ldx, a multiple of 8, 16-byte aligned), W [L, H] bf16 contiguous (16-byte aligned), b [L] ->
+ *        logits [R, L] contiguous:  logits[r, l] = sum_c x[r,c] * keep[r,c] * scale * W[l,c] + b[l], fp32 accumulation in a fixed
+ *        order per row (a row's logits depend on that row alone), rounded once.
+ *   bwd: dlogits [R, L] contiguous -> dx [R, H] bf16 contiguous, dx[r,c] = keep[r,c] * scale * sum_l dlogits[r,l] * W[l,c];
+ *        dW [L, H] and db [L]: fp32 sums over rows, per-slab partials in `part` (dle_cls_head_bwd_partials(R) * L * (H + 1) floats)
+ *        summed in a fixed order by the colsum finalize kernel -- deterministic, no atomics; a row whose dlogits are 0 adds exactly 0.
+ *        The keep bits are recomputed (nothing is stored), so backward sees forward's mask.
+ * keep[r,c] is the hidden-dropout bit of flat element r*H + c under (seed, dropout_stream), as at every other hidden-dropout site
+ * (dropout_keep8 of common.cuh, the step counter seed_dev mixed in when non-NULL), scale = 1/(1-p); p = 0 keeps everything.
+ * dtype (DLE_DTYPE_BF16 or DLE_DTYPE_F32) is that of b, logits, dlogits, dW and db: the parameter dtype.  1 <= L <= 32, H % 32 == 0,
+ * 1 <= R <= 2097120, 0 <= p < 1; anything else returns DLE_ERR_INVALID before any CUDA call.  No host work: graph-capturable. */
+int dle_cls_head_fwd(const void* x, int64_t ldx, const void* w, const void* b, int32_t R, int32_t H, int32_t L, int32_t dtype,
+                     float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, void* logits, void* stream);
+int dle_cls_head_bwd_partials(int32_t R);
+int dle_cls_head_bwd(const void* dlogits, const void* x, int64_t ldx, const void* w, int32_t R, int32_t H, int32_t L, int32_t dtype,
+                     float dropout_p, uint64_t seed, const uint64_t* seed_dev, uint32_t dropout_stream, void* dx, float* part,
+                     void* dw, void* db, void* stream);
 /* masked-row gather (dense sequence output): out[i,:] = x[idx[i],:]  -- bit exact.
  * replaces torch.index_select at modeling.py:590.  bwd scatters rows back (rows are unique).
  * idx[i] == -1 marks a PADDING slot of a static-size index list (torch.nonzero_static): gather writes a zero row, scatter skips it;
