@@ -961,3 +961,48 @@ class BertForSequenceClassification(BertPreTrainedModel):
                 self.distill_state_dict["pred_states"] = final_output
             if not self.distillation or not self.training:
                 return final_output
+
+
+class BertForMultipleChoice(BertPreTrainedModel):
+    """Multiple-choice head over the pooled output (reference modeling.py:1158-1224): one score per choice, classifier(dropout(pooled))
+    with classifier = nn.Linear(H, 1), and a softmax over an example's num_choices scores.
+    forward(input_ids, token_type_ids=None, attention_mask=None, labels=None) with inputs [B, num_choices, S] -> the mean
+    cross-entropy (fp32) when labels [B] are given, else reshaped_logits [B, num_choices] in the parameter dtype.
+
+    The dropout and the classifier run as ops.ClassifierHeadFn with L = 1, keyed like BertForSequenceClassification's head.  With
+    pack_sequences(k), k a multiple of num_choices, the inputs are [B, S] rows of the packed SWAG format (packing.py): attention_mask
+    holds sample numbers, the m-th example of a row fills slots m*C .. m*C + C-1 with its choices in order, and labels is [B*k/C] with
+    -100 for an empty group.  The pooled output is [B*k, H], so the reference's own view(-1, num_choices) lines each example's scores
+    up with its label and the forward below runs unchanged."""
+
+    def __init__(self, config, num_choices):
+        super().__init__(config)
+        self.num_choices = num_choices
+        self.bert = BertModel(config)
+        self.dropout = nn.Dropout(config.hidden_dropout_prob)
+        self.classifier = nn.Linear(config.hidden_size, 1)
+        self.apply(self.init_bert_weights)
+        self._stream_id = ops.new_stream_id()
+
+    def pack_sequences(self, max_per_row):
+        """As BertPreTrainedModel.pack_sequences, but max_per_row counts sample slots, num_choices per example: it must be a multiple
+        of num_choices (0 or None turns packing off), so that every example's choices fill whole, aligned groups of slots."""
+        k = int(max_per_row or 0)
+        if k < 0 or k % self.num_choices != 0:
+            raise L.DleError(f"pack_sequences on BertForMultipleChoice takes a positive multiple of num_choices = "
+                             f"{self.num_choices} (0 or None turns packing off), got {max_per_row}")
+        super().pack_sequences(k)
+
+    def forward(self, input_ids, token_type_ids=None, attention_mask=None, labels=None):
+        flat_input_ids = input_ids.view(-1, input_ids.size(-1))
+        flat_token_type_ids = None if token_type_ids is None else token_type_ids.view(-1, token_type_ids.size(-1))
+        flat_attention_mask = None if attention_mask is None else attention_mask.view(-1, attention_mask.size(-1))
+        _, pooled_output = self.bert(flat_input_ids, flat_token_type_ids, flat_attention_mask)
+        p = self.dropout.p if self.dropout.training else 0.0
+        x = pooled_output if pooled_output.dtype == bf16 else pooled_output.to(bf16)
+        logits = ops.ClassifierHeadFn.apply(x, self.classifier.weight, self.classifier.bias, p, self._stream_id)
+        reshaped_logits = logits.view(-1, self.num_choices)
+
+        if labels is not None:
+            return nn.CrossEntropyLoss()(reshaped_logits.float(), labels)      # fp32 on the 16-bit logits, as glue.glue_loss
+        return reshaped_logits

@@ -29,6 +29,20 @@ The packed GLUE format (BertForSequenceClassification.pack_sequences(k); the key
     reference's CrossEntropyLoss (run_glue.py:597), so its loss line runs unchanged and averages over the real samples.
   * example_index (a host attribute of the PackedBatch, numpy int64 [B*k]): the index of the example in each slot, -1 when the slot
     is empty.  Evaluation maps the [B*k, num_labels] logits back to their examples through it.
+
+The packed SWAG format (BertForMultipleChoice.pack_sequences(k), k a multiple of the number of choices C; the keys
+swag.swag_training_step reads).  The unpacked source is run_swag.py's batch (select_field, :237-245, :548-552): input_ids, input_mask,
+segment_ids [N, C, S_choice], each choice a right-padded [CLS] context [SEP] ending [SEP] row, and label_ids [N].  The unit of packing
+is the example, never a single choice: a row holds at most k/C whole examples, each choice keeping its own tokens and segment ids and
+the choices in their order (the label indexes them).
+
+  * input_ids, segment_ids: int64 [B, S].
+  * input_mask: int64 [B, S].  Choice c of the row's m-th example holds sample number m*C + c + 1; the tail holds 0.  Every sample
+    number is a slot of attention_mask above, so the pooled output is [B*k, H] and slot b*k + m*C + c is choice c of that example.
+  * label_ids: int64 [B*k/C].  Group b*(k/C) + m holds the label of the m-th example of row b, -100 when the group is empty.  The
+    reference's view(-1, C) of the [B*k, 1] logits therefore lines every group of C scores up with its label.
+  * example_index (a host attribute of the PackedBatch, numpy int64 [B*k/C]): the index of the example in each group, -1 when the
+    group is empty.
 """
 import numpy as np
 import torch
@@ -78,9 +92,23 @@ class GlueSample:
         return len(self.input_ids)
 
 
+class SwagSample:
+    """One SWAG example: per choice, the ids and segment ids of its real tokens (tuples of C 1-D int64 numpy arrays, in choice order),
+    its label and the index of the example in its source stream.  Its length is the sum of its choices' lengths."""
+    __slots__ = ("input_ids", "segment_ids", "label", "example_index")
+    n_labels = 0                                         # no MLM labels: pack()'s label bound never binds
+
+    def __init__(self, input_ids, segment_ids, label, example_index):
+        self.input_ids, self.segment_ids = tuple(input_ids), tuple(segment_ids)
+        self.label, self.example_index = int(label), int(example_index)
+
+    def __len__(self):
+        return sum(len(c) for c in self.input_ids)
+
+
 class PackedBatch(dict):
-    """A packed batch: the tensors as dict items, and `num_samples`, the number of samples it holds (a host int).  A SQuAD batch also
-    carries `feature_index`, a GLUE batch `example_index` (see the module docstring)."""
+    """A packed batch: the tensors as dict items, and `num_samples`, the number of samples it holds (a host int; a SWAG batch counts
+    examples).  A SQuAD batch also carries `feature_index`, a GLUE or SWAG batch `example_index` (see the module docstring)."""
 
     def __init__(self, tensors, num_samples):
         super().__init__(tensors)
@@ -300,6 +328,90 @@ def unpack_glue(batch):
     return out
 
 
+SWAG_KEYS = ("input_ids", "input_mask", "segment_ids", "label_ids")
+
+
+def _check_choices(k, num_choices):
+    if num_choices < 1 or k < 1 or k % num_choices != 0:
+        raise ValueError(f"max_per_row must be a positive multiple of num_choices = {num_choices}, got {k}")
+
+
+def split_swag_samples(batch, first_example_index=0):
+    """The examples of an unpacked SWAG batch (input_ids, input_mask, segment_ids [N, C, S_choice] with right-padded 0/1 masks,
+    label_ids [N]): per choice the tokens whose mask is 1, example index first_example_index + n.  An example none of whose choices
+    holds a token holds no example; one with some empty choices raises ValueError (its scores would not line up with its label)."""
+    ids, am, seg, lab = (batch[key].cpu().numpy() for key in SWAG_KEYS)
+    if am.ndim != 3:
+        raise ValueError(f"split_swag_samples takes [N, C, S] tensors, got input_mask of shape {tuple(am.shape)}")
+    if am.min(initial=0) < 0 or am.max(initial=0) > 1:
+        raise ValueError("split_swag_samples takes an unpacked batch: input_mask must hold only 0 and 1")
+    out = []
+    for n in range(ids.shape[0]):
+        keep = am[n] != 0
+        has = keep.any(-1)
+        if not has.any():
+            continue
+        if not has.all():
+            raise ValueError(f"example {first_example_index + n}: choices {np.nonzero(~has)[0].tolist()} hold no token")
+        out.append(SwagSample([ids[n, c][keep[c]] for c in range(ids.shape[1])], [seg[n, c][keep[c]] for c in range(ids.shape[1])],
+                              lab[n], first_example_index + n))
+    return out
+
+
+def to_swag_batch(samples, rows, B, S, k, num_choices, pin=False):
+    """The packed SWAG batch (PackedBatch of CPU int64 tensors, with example_index) with the examples rows[r] in row r; rows past
+    len(rows) and groups past a row's examples are empty (label -100, example index -1).  ValueError when k is not a positive multiple
+    of num_choices, or a row exceeds S tokens or k/num_choices examples, or an example does not hold num_choices choices."""
+    _check_choices(k, num_choices)
+    C, E = num_choices, k // num_choices
+    ids = np.zeros((B, S), np.int64)
+    seg = np.zeros((B, S), np.int64)
+    am = np.zeros((B, S), np.int64)
+    lab = np.full(B * E, GLUE_IGNORE, np.int64)
+    ei = np.full(B * E, -1, np.int64)
+    if len(rows) > B:
+        raise ValueError(f"{len(rows)} rows do not fit a batch of {B}")
+    count = 0
+    for r, members in enumerate(rows):
+        n_row = sum(len(samples[i]) for i in members)
+        if n_row > S or len(members) > E:
+            raise ValueError(f"row {r}: {len(members)} examples of {n_row} tokens do not fit a row of {E} examples and {S} tokens")
+        off = 0
+        for m, i in enumerate(members):
+            s = samples[i]
+            if len(s.input_ids) != C:
+                raise ValueError(f"example {s.example_index} holds {len(s.input_ids)} choices, not {C}")
+            for c in range(C):
+                n = len(s.input_ids[c])
+                ids[r, off:off + n] = s.input_ids[c]
+                seg[r, off:off + n] = s.segment_ids[c]
+                am[r, off:off + n] = m * C + c + 1
+                off += n
+            lab[r * E + m] = s.label
+            ei[r * E + m] = s.example_index
+            count += 1
+    t = {key: torch.from_numpy(v) for key, v in zip(SWAG_KEYS, (ids, am, seg, lab))}
+    if pin:
+        t = {key: v.pin_memory() for key, v in t.items()}
+    batch = PackedBatch(t, count)
+    batch.example_index = ei
+    return batch
+
+
+def unpack_swag(batch, num_choices):
+    """The examples of a packed SWAG batch in group order (the inverse of to_swag_batch)."""
+    ids, am, seg, lab = (batch[key].cpu().numpy() for key in SWAG_KEYS)
+    C, E = num_choices, lab.shape[0] // ids.shape[0]
+    out = []
+    for r in range(ids.shape[0]):
+        for m in range(E):
+            sels = [am[r] == m * C + c + 1 for c in range(C)]
+            if any(sel.any() for sel in sels):
+                g = r * E + m
+                out.append(SwagSample([ids[r][sel] for sel in sels], [seg[r][sel] for sel in sels], lab[g], batch.example_index[g]))
+    return out
+
+
 def token_fill(batch):
     """Share of the batch's B*S token slots that hold a sample token."""
     am = batch["input_mask"] if "input_mask" in batch else batch["attention_mask"]
@@ -314,15 +426,21 @@ class PackedLoader:
 
     squad=True packs unpacked SQuAD batches (SQUAD_KEYS, 0/1 input_mask) into the packed SQuAD format instead; max_pred is unused
     then, and feature indices count the source's rows from 0.  glue=True does the same for unpacked GLUE batches (GLUE_KEYS) and
-    the packed GLUE format, with example indices counting the source's rows from 0."""
+    the packed GLUE format, with example indices counting the source's rows from 0.  swag=True packs unpacked SWAG batches
+    (SWAG_KEYS, [N, C, S_choice]) into the packed SWAG format: whole examples of num_choices choices, at most max_per_row /
+    num_choices of them per row (max_per_row counts sample slots and must be a multiple of num_choices)."""
 
-    def __init__(self, source, batch_size, seq_len, max_per_row, max_pred=0, pool_rows=2, pin=False, squad=False, glue=False):
+    def __init__(self, source, batch_size, seq_len, max_per_row, max_pred=0, pool_rows=2, pin=False, squad=False, glue=False,
+                 swag=False, num_choices=4):
         if max_per_row < 1:
             raise ValueError(f"max_per_row must be >= 1, got {max_per_row}")
-        if squad and glue:
-            raise ValueError("PackedLoader packs one format: pass squad=True or glue=True, not both")
+        if squad + glue + swag > 1:
+            raise ValueError("PackedLoader packs one format: pass one of squad=True, glue=True or swag=True")
+        if swag:
+            _check_choices(max_per_row, num_choices)
         self.source, self.B, self.S, self.k, self.P = source, batch_size, seq_len, max_per_row, max_pred
         self.pool_tokens, self.pin, self.squad, self.glue = pool_rows * batch_size * seq_len, pin, squad, glue
+        self.swag, self.C = swag, num_choices
 
     def __iter__(self):
         pool, it, done = [], iter(self.source), False
@@ -335,8 +453,9 @@ class PackedLoader:
                 except StopIteration:
                     done = True
                     break
-                if self.squad or self.glue:
-                    new = (split_squad_samples if self.squad else split_glue_samples)(batch, rows_seen)
+                if self.squad or self.glue or self.swag:
+                    split = split_squad_samples if self.squad else split_glue_samples if self.glue else split_swag_samples
+                    new = split(batch, rows_seen)
                     rows_seen += batch["input_ids"].shape[0]
                 else:
                     new = split_samples(batch, self.P)
@@ -344,9 +463,13 @@ class PackedLoader:
                 tokens += sum(len(s) for s in new)
             if not pool:
                 return
-            rows, unplaced = pack(pool, self.B, self.S, self.k, self.P)
-            fmt = to_squad_batch if self.squad else to_glue_batch if self.glue else to_batch
-            yield fmt(pool, rows, self.B, self.S, self.k, self.pin)
+            if self.swag:
+                rows, unplaced = pack(pool, self.B, self.S, self.k // self.C, self.P)
+                yield to_swag_batch(pool, rows, self.B, self.S, self.k, self.C, self.pin)
+            else:
+                rows, unplaced = pack(pool, self.B, self.S, self.k, self.P)
+                fmt = to_squad_batch if self.squad else to_glue_batch if self.glue else to_batch
+                yield fmt(pool, rows, self.B, self.S, self.k, self.pin)
             pool = [pool[i] for i in unplaced]
 
 

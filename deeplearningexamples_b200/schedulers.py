@@ -42,10 +42,15 @@ class LinearWarmUpScheduler(_LRScheduler):
     """Linear warm-up to the base rate over `warmup` (a fraction of total_steps), then linear decay to zero at total_steps -- the
     schedule of the SQuAD fine-tuning driver (reference schedulers.py:90-106, used at run_squad.py:1014-1016).
     Host-side by default, like the reference.  With `device` set the schedule is evaluated on the device from the optimizer's own
-    step counter (as PolyWarmUpScheduler does), writing the lr tensor in place: no host value is baked into a captured CUDA graph."""
+    step counter (as PolyWarmUpScheduler does), writing the lr tensor in place: no host value is baked into a captured CUDA graph.
 
-    def __init__(self, optimizer, warmup, total_steps, last_epoch=-1, device=None, base_lr=None):
+    The n-th step (n = 0, 1, ...) runs at progress (n + progress_offset) / total_steps.  The default 1 is the schedule above;
+    progress_offset=0 is the SWAG driver's base * warmup_linear(global_step / t_total) (run_swag.py:486-493, optimization.py:46-49),
+    whose first step runs at lr 0."""
+
+    def __init__(self, optimizer, warmup, total_steps, last_epoch=-1, device=None, base_lr=None, progress_offset=1):
         self.warmup, self.total_steps = float(warmup), float(total_steps)
+        self.progress_offset = float(progress_offset)
         self.device = device
         if device is not None:
             self._base = torch.tensor(float(base_lr if base_lr is not None else 1.0), device=device)
@@ -55,7 +60,7 @@ class LinearWarmUpScheduler(_LRScheduler):
         if self.device is not None:
             group0 = self.optimizer.param_groups[0]
             step_t = group0['step'] if isinstance(group0.get('step'), torch.Tensor) else torch.zeros(1, dtype=torch.int32, device=self.device)
-            progress = (step_t.reshape(()).float() + 1.0) / self.total_steps
+            progress = (step_t.reshape(()).float() + self.progress_offset) / self.total_steps
             factor = torch.where(progress < self.warmup, progress / self.warmup,
                                  torch.clamp((progress - 1.0) / (self.warmup - 1.0), min=0.0))
             lr = self._base * factor
@@ -71,7 +76,8 @@ class LinearWarmUpScheduler(_LRScheduler):
             group['lr'] = lr
 
     def get_lr(self):
-        progress = self.last_epoch / self.total_steps
+        # last_epoch is 0 after construction and n + 1 at the n-th step(); the initial rate is the first step's at offset 0
+        progress = max(self.last_epoch - 1.0 + self.progress_offset, 0.0) / self.total_steps
         if progress < self.warmup:
             factor = progress / self.warmup
         else:

@@ -12,9 +12,9 @@ import sys
 
 from deeplearningexamples_b200.modeling import *  # noqa: F401,F403
 from deeplearningexamples_b200 import modeling as _m
-from deeplearningexamples_b200.modeling import (ACT2FN, BertConfig, BertEmbeddings, BertEncoder, BertForPreTraining,  # noqa: F401
-                                                BertForQuestionAnswering, BertForSequenceClassification, BertLayer, BertModel,
-                                                BertPreTrainedModel, LinearActivation, gelu)
+from deeplearningexamples_b200.modeling import (ACT2FN, BertConfig, BertEmbeddings, BertEncoder, BertForMultipleChoice,  # noqa: F401
+                                                BertForPreTraining, BertForQuestionAnswering, BertForSequenceClassification, BertLayer,
+                                                BertModel, BertPreTrainedModel, LinearActivation, gelu)
 
 
 def _driver_flag(name, default):
