@@ -80,6 +80,15 @@ SIGNATURES = {
     "dle_lamb_step": (_i32, [_vp, _vp, _f32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "dle_lamb_grad_norm": (_i32, [_vp, _vp, _vp, _vp]),
     "dle_adam_step": (_i32, [_vp, _vp, _f32, _f32, _i32, _vp, _vp, _vp]),
+    "dle_relkl_partials": (_i32, [_i32, _i32, _i32]),
+    "dle_relkl_fwd": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _f32, _f32, _i32, _i32, _i32, _i32, _i32, _f32, _vp, _vp,
+                             _vp, _vp, _vp]),
+    "dle_relkl_bwd": (_i32, [_vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _f32, _f32, _i32, _i32, _i32, _i32, _i32, _vp, _vp, _vp,
+                             _f32, _vp, _vp, _vp, _i64, _vp]),
+    "dle_cosine_rows_partials": (_i32, [_i64]),
+    "dle_cosine_rows_fwd": (_i32, [_vp, _i64, _vp, _i64, _i64, _i32, _vp, _vp, _vp]),
+    "dle_cosine_rows_bwd": (_i32, [_vp, _i64, _vp, _i64, _i64, _i32, _vp, _vp, _i64, _vp]),
+    "dle_add_rows_bf16": (_i32, [_vp, _i64, _vp, _i64, _i64, _i32, _vp, _vp]),
 }
 
 _ERRORS = {-22: "DLE_ERR_INVALID (bad shape/alignment/null pointer)", -5: "DLE_ERR_CUDA (launch/driver failure)",

@@ -14,7 +14,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.dirname(HERE)
 OUT = os.path.join(PKG, "libdle_b200.so")
 OBJ_DIR = os.path.join(HERE, "build")
-SOURCES = ["gemm_sm90.cu", "attention_sm90.cu", "lamb.cu", "pointwise.cu", "loss.cu"]
+SOURCES = ["gemm_sm90.cu", "attention_sm90.cu", "lamb.cu", "pointwise.cu", "loss.cu", "distill_sm90.cu"]
 HEADERS = [os.path.join(HERE, "common.cuh"), os.path.join(os.path.dirname(PKG), "include", "dle_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

@@ -483,3 +483,91 @@ def cast_bf16_to_f32(x, out=None):
     out = torch.empty(x.shape, device=x.device, dtype=torch.float32) if out is None else out
     L.launch_count["n"] += 1; L.check(lib.dle_cast_bf16_to_f32(_ptr(x), _ptr(out), x.numel(), _stream()), "dle_cast_bf16_to_f32")
     return out
+
+
+# ------------------------------------------------------------------------------------------------
+# distillation losses (csrc/distill_sm90.cu)
+# ------------------------------------------------------------------------------------------------
+def _head_block(t, A, name):
+    """A 2-D bf16 view whose first 64*A columns are the heads' blocks (last dim contiguous); returns its row stride."""
+    _req(t, bf16, name)
+    ld = _row_major_2d(t, name)
+    if t.shape[1] < 64 * A:
+        raise L.DleError(f"{name} has {t.shape[1]} columns, fewer than 64 * A = {64 * A}")
+    return ld
+
+
+def relkl_fwd(xs, ys, xt, yt, mask_s, mask_t, B, S, A, scale_s, scale_t, where_rule, seq_first, norm):
+    """loss = norm * sum over rows of KL(softmax(t) || softmax(s)); s / t = scale * X Y^T (+ mask) per (b, h) (see dle_relkl_fwd).
+    xs, ys, xt, yt: 2-D bf16 views starting at head 0's column block; masks fp32 [B, S] or None.  Returns (loss [] fp32, lse_s,
+    lse_t [B, A, S])."""
+    lib = L.load()
+    ld_s, ld_t = _head_block(xs, A, "xs"), _head_block(xt, A, "xt")
+    if _head_block(ys, A, "ys") != ld_s or _head_block(yt, A, "yt") != ld_t:
+        raise L.DleError("X and Y of one model must share a row stride")
+    for m, n in ((mask_s, "mask_s"), (mask_t, "mask_t")):
+        if m is not None:
+            _req(m, torch.float32, n)
+    dev = xs.device
+    lse_s = torch.empty((B, A, S), device=dev, dtype=torch.float32)
+    lse_t = torch.empty((B, A, S), device=dev, dtype=torch.float32)
+    n_part = lib.dle_relkl_partials(B, S, A)
+    L.check(n_part if n_part < 0 else 0, "dle_relkl_partials")
+    ws = torch.empty(n_part + 1, device=dev, dtype=torch.float32)
+    L.launch_count["n"] += 2; L.check(lib.dle_relkl_fwd(_ptr(xs), _ptr(ys), _ptr(xt), _ptr(yt), ld_s, ld_t, _ptr(mask_s), _ptr(mask_t),
+                                                        scale_s, scale_t, 1 if where_rule else 0, B, S, A, 1 if seq_first else 0, norm,
+                                                        _ptr(lse_s), _ptr(lse_t), _ptr(ws[1:]), _ptr(ws), _stream()), "dle_relkl_fwd")
+    return ws[0], lse_s, lse_t
+
+
+def relkl_bwd(xs, ys, xt, yt, mask_s, mask_t, B, S, A, scale_s, scale_t, where_rule, seq_first, lse_s, lse_t, grad_scale, norm, dx, dy,
+              dzero=None):
+    """Gradient of relkl_fwd's loss times grad_scale (fp32 device scalar) into the bf16 views dx (= dS Y_s) and dy (= dS^T X_s); when
+    dx and dy are the same view (X = Y) the two terms are summed.  dzero: a view zero-filled per head block, or None."""
+    lib = L.load()
+    ld_s, ld_t = _head_block(xs, A, "xs"), _head_block(xt, A, "xt")
+    ld_d = _head_block(dx, A, "dx")
+    if _head_block(dy, A, "dy") != ld_d or (dzero is not None and _head_block(dzero, A, "dzero") != ld_d):
+        raise L.DleError("dx, dy and dzero must share a row stride")
+    L.launch_count["n"] += 2; L.check(lib.dle_relkl_bwd(_ptr(xs), _ptr(ys), _ptr(xt), _ptr(yt), ld_s, ld_t, _ptr(mask_s), _ptr(mask_t),
+                                                        scale_s, scale_t, 1 if where_rule else 0, B, S, A, 1 if seq_first else 0,
+                                                        _ptr(lse_s), _ptr(lse_t), _ptr(_req(grad_scale, torch.float32, "grad_scale")),
+                                                        norm, _ptr(dx), _ptr(dy), _ptr(dzero), ld_d, _stream()), "dle_relkl_bwd")
+
+
+def cosine_rows_fwd(x, y):
+    """mean over rows of 1 - cos(x_r, y_r) (torch's CosineEmbeddingLoss with target 1) on bf16 [rows, H]; returns a [] fp32 tensor."""
+    lib = L.load()
+    _req(x, bf16, "x"); _req(y, bf16, "y")
+    if x.shape != y.shape or x.dim() != 2:
+        raise L.DleError(f"cosine rows need two [rows, H] tensors of one shape, got {tuple(x.shape)} and {tuple(y.shape)}")
+    rows, H = x.shape
+    n_part = lib.dle_cosine_rows_partials(rows)
+    L.check(n_part if n_part < 0 else 0, "dle_cosine_rows_partials")
+    ws = torch.empty(n_part + 1, device=x.device, dtype=torch.float32)
+    L.launch_count["n"] += 2; L.check(lib.dle_cosine_rows_fwd(_ptr(x), _row_major_2d(x, "x"), _ptr(y), _row_major_2d(y, "y"), rows, H,
+                                                              _ptr(ws[1:]), _ptr(ws), _stream()), "dle_cosine_rows_fwd")
+    return ws[0]
+
+
+def cosine_rows_bwd(x, y, grad_scale):
+    """dx (bf16 [rows, H]) of cosine_rows_fwd's loss times grad_scale (fp32 device scalar)."""
+    lib = L.load()
+    rows, H = x.shape
+    dx = torch.empty((rows, H), device=x.device, dtype=bf16)
+    L.launch_count["n"] += 1; L.check(lib.dle_cosine_rows_bwd(_ptr(x), _row_major_2d(x, "x"), _ptr(y), _row_major_2d(y, "y"), rows, H,
+                                                              _ptr(_req(grad_scale, torch.float32, "grad_scale")), _ptr(dx), H, _stream()),
+                                      "dle_cosine_rows_bwd")
+    return dx
+
+
+def add_rows_bf16(dst, src, colsum=None):
+    """dst += src (bf16 2-D views of one shape, fp32 add); colsum (fp32 [cols]) += column sums of src when given."""
+    lib = L.load()
+    _req(dst, bf16, "dst"); _req(src, bf16, "src")
+    if dst.shape != src.shape:
+        raise L.DleError(f"add_rows_bf16: shapes differ, {tuple(dst.shape)} and {tuple(src.shape)}")
+    if colsum is not None:
+        _req(colsum, torch.float32, "colsum")
+    L.launch_count["n"] += 1; L.check(lib.dle_add_rows_bf16(_ptr(dst), _row_major_2d(dst, "dst"), _ptr(src), _row_major_2d(src, "src"),
+                                                            dst.shape[0], dst.shape[1], _ptr(colsum), _stream()), "dle_add_rows_bf16")

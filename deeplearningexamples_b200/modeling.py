@@ -219,6 +219,40 @@ class BertEmbeddings(nn.Module):
         return embeddings
 
 
+class AttentionScores:
+    """The pre-softmax attention scores QK^T/sqrt(d) + mask [B, A, S, S] of one layer (reference modeling.py:349-357, cached at :380-381),
+    as a handle: the fused kernel never forms them, so this holds what they are computed from -- the layer's packed qkv [T, 3H]
+    (an autograd output of the layer), the fp32 additive mask [B, S], the head count, the 1/sqrt(64) scale and the token order.
+    distill.TransformerLosses sends a student / teacher pair to the relation-KL kernel.  materialize() forms the tensor, for tests
+    and debugging only."""
+
+    def __init__(self, qkv, mask, B, S, A, seq_first, scale=0.125):
+        self.qkv, self.mask, self.B, self.S, self.A, self.seq_first, self.scale = qkv, mask, B, S, A, seq_first, scale
+
+    @property
+    def shape(self):
+        return torch.Size((self.B, self.A, self.S, self.S))
+
+    def size(self, dim=None):
+        return self.shape if dim is None else self.shape[dim]
+
+    def detach(self):
+        return AttentionScores(self.qkv.detach(), self.mask, self.B, self.S, self.A, self.seq_first, self.scale)
+
+    def materialize(self):
+        """fp32 [B, A, S, S] scores (with the mask added), differentiable through qkv."""
+        B, S, A = self.B, self.S, self.A
+        H = A * 64
+        q = self.qkv.float()
+        q = q.view(S, B, 3 * H).transpose(0, 1) if self.seq_first else q.view(B, S, 3 * H)
+        qh = q[..., :H].reshape(B, S, A, 64).permute(0, 2, 1, 3)
+        kh = q[..., H:2 * H].reshape(B, S, A, 64).permute(0, 2, 1, 3)
+        scores = torch.matmul(qh, kh.transpose(-1, -2)) * self.scale
+        if self.mask is not None:
+            scores = scores + self.mask.view(B, 1, 1, S)
+        return scores
+
+
 class BertSelfAttention(nn.Module):
     """Multi-head self-attention (reference modeling.py:304-384).  The three nn.Linear parameters keep their
     checkpoint names but live in ONE packed [3H,H] / [3H] storage, so a single GEMM produces q|k|v."""
@@ -361,9 +395,14 @@ class BertLayer(nn.Module):
 
     def _fusable(self):
         att = self.attention.self
-        return (not self.distillation and not att.distillation and att.attention_head_size == 64
+        return (att.attention_head_size == 64
                 and self.intermediate.dense_act.act == "gelu" and self.intermediate.dense_act.bias is not None
                 and not getattr(self, "force_modular", False))
+
+    def _distill_states(self):
+        """True when this layer records attention scores or value states for distillation."""
+        att = self.attention.self
+        return att.distillation and (att.distill_config["use_attention_scores"] or att.distill_config["use_value_states"])
 
     def forward(self, hidden_states, attention_mask):
         """hidden_states (seq, bsz, hidden) -> (seq, bsz, hidden).  Default: one hand-differentiated autograd node for
@@ -377,11 +416,25 @@ class BertLayer(nn.Module):
             tr = self.training
             cfg = (B, S, att.num_attention_heads, att.dropout.p if tr else 0.0, so.dropout.p if tr else 0.0, so.LayerNorm.eps,
                    att._stream_id, so._stream_id, out._stream_id, not transposed)
-            y = ops.BertLayerFn.apply(x2, mask, att.query.weight, att.key.weight, att.value.weight, att.query.bias, att.key.bias,
-                                      att.value.bias, so.dense.weight, so.dense.bias, so.LayerNorm.weight, so.LayerNorm.bias,
-                                      it.weight, it.bias, out.dense.weight, out.dense.bias, out.LayerNorm.weight, out.LayerNorm.bias,
-                                      w_qkv, b_qkv, cfg)
-            return restore(y)
+            args = (x2, mask, att.query.weight, att.key.weight, att.value.weight, att.query.bias, att.key.bias,
+                    att.value.bias, so.dense.weight, so.dense.bias, so.LayerNorm.weight, so.LayerNorm.bias,
+                    it.weight, it.bias, out.dense.weight, out.dense.bias, out.LayerNorm.weight, out.LayerNorm.bias,
+                    w_qkv, b_qkv, cfg)
+            if not self._distill_states():
+                y = restore(ops.BertLayerFn.apply(*args))
+            else:
+                # the fused kernel never forms the scores: the layer hands out qkv and the attention output instead, and the
+                # distillation losses (distill.py) compute from those (reference modeling.py:378-383)
+                y, qkv, ctx = ops.BertLayerDistillFn.apply(*args)
+                y = restore(y)
+                if att.distill_config["use_attention_scores"]:
+                    att.distill_state_dict["attention_scores"] = AttentionScores(qkv, mask, B, S, att.num_attention_heads,
+                                                                                 not transposed)
+                if att.distill_config["use_value_states"]:
+                    att.distill_state_dict["value_states"] = restore(ctx)
+            if self.distillation and self.distill_config["use_hidden_states"]:
+                self.distill_state_dict["hidden_states"] = y
+            return y
         attention_output = self.attention(hidden_states, attention_mask)
         intermediate_output = self.intermediate(attention_output)
         layer_output = self.output(intermediate_output, attention_output)
@@ -395,7 +448,7 @@ class BertLayer(nn.Module):
         of 64 from max_seqlen to 512; the padded length S rounded up to 64) keys the attention masks, so that a right-padded batch draws
         the padded path's attention keep bits.  Otherwise the inference forward: no dropout and no autograd.  Either way a valid row
         gets forward's result under a 0 / -10000 mask when dropout is off."""
-        if not self._fusable():
+        if not self._fusable() or self.distillation or self.attention.self.distillation:
             raise L.DleError("the padding-free route needs the fused layer (head size 64, gelu with bias, no distillation)")
         att, so, it, out = self.attention.self, self.attention.output, self.intermediate.dense_act, self.output
         w_qkv, b_qkv = att._packed()
@@ -563,6 +616,48 @@ class BertPreTrainingHeads(nn.Module):
                              "loss; raise --max_predictions_per_seq or unset static_masked_count" % int(self.static_masked_count))
 
 
+def _apply_distill_config(config, distill_config, pooler):
+    """Merge a distillation config (JSON path or dict with "distillation" and "distillation_config") into `config`, setting
+    distillation_config["use_pooler"] = pooler (reference modeling.py:644-648)."""
+    if not distill_config:
+        return
+    if isinstance(distill_config, dict):
+        d = copy.deepcopy(distill_config)
+    else:
+        with open(distill_config, "r") as fh:
+            d = json.load(fh)
+    d["distillation_config"]["use_pooler"] = pooler
+    config.__dict__.update(d)
+
+
+class Project(nn.Module):
+    """nn.Linear(H_student, H_teacher) applied to each tensor of a list: projects student states to the teacher's width
+    (reference modeling.py:1373-1407; same init, same state-dict keys `fit_dense.weight` / `fit_dense.bias`)."""
+
+    def __init__(self, student_config, teacher_config):
+        super().__init__()
+        self.student_config = student_config
+        self.teacher_config = teacher_config
+        self.fit_dense = nn.Linear(student_config.hidden_size, teacher_config.hidden_size)
+        self.apply(self.init_weights)
+
+    def forward(self, student_tensor_list):
+        out = []
+        for t in student_tensor_list:                  # the GEMM with its bias epilogue (ops.LinearFn), token order kept
+            x2, restore, _ = _tokens(t)
+            out.append(restore(ops.LinearFn.apply(x2, self.fit_dense.weight, self.fit_dense.bias, None)))
+        return out
+
+    def init_weights(self, module):
+        if isinstance(module, (nn.Linear, nn.Embedding)):
+            module.weight.data.normal_(mean=0.0, std=self.student_config.initializer_range)
+        elif isinstance(module, nn.LayerNorm):
+            module.bias.data.zero_()
+            module.weight.data.fill_(1.0)
+        if isinstance(module, nn.Linear) and module.bias is not None:
+            module.bias.data.zero_()
+
+
 class BertPreTrainedModel(nn.Module):
     """Weight initialisation + flags shared by the task models (reference modeling.py:598-636)."""
 
@@ -630,6 +725,17 @@ class BertPreTrainedModel(nn.Module):
                          ("pooler.dense.", "pooler.dense_act."))
 
     @classmethod
+    def from_scratch(cls, pretrained_model_name_or_path, distill_config=None, pooler=True, *inputs, **kwargs):
+        """A freshly initialised model from the config file in a directory (reference modeling.py:638-652): `config.json` (the
+        reference's name) or `bert_config.json`; `distill_config` as in from_pretrained.  Returns (model, config)."""
+        import os
+        root = str(pretrained_model_name_or_path)
+        name = "config.json" if os.path.exists(os.path.join(root, "config.json")) else "bert_config.json"
+        config = BertConfig.from_json_file(os.path.join(root, name))
+        _apply_distill_config(config, distill_config, pooler)
+        return cls(config, *inputs, **kwargs), config
+
+    @classmethod
     def from_pretrained(cls, pretrained_model_name_or_path, state_dict=None, cache_dir=None, from_tf=False, distill_config=None,
                         pooler=True, *inputs, **kwargs):
         """Build the model from a local pretrained archive and load its weights: the fine-tuning entry of the reference
@@ -640,8 +746,9 @@ class BertPreTrainedModel(nn.Module):
         gamma/beta -> weight/bias, `intermediate.dense.` / `pooler.dense.` -> `..dense_act.`), a `bert.` prefix is dropped when this
         class has no `bert` attribute (loading a pretraining checkpoint into `BertModel`), missing and unused keys are logged, shape
         mismatches raise.  Not carried over: model names that resolve to downloads (no network: the reference logs an error and
-        returns None for an unknown name, and so does this), TensorFlow checkpoints (`from_tf`) and the distillation config
-        (out of scope, DESIGN.md section 7) -- both raise NotImplementedError."""
+        returns None for an unknown name, and so does this) and TensorFlow checkpoints (`from_tf`, raises NotImplementedError).
+        `distill_config` (a JSON path or dict, e.g. distillation_config_backbone.json) is merged into the config as the reference does
+        (modeling.py:719-722), with `use_pooler = pooler`."""
         import logging
         import os
         import shutil
@@ -650,8 +757,6 @@ class BertPreTrainedModel(nn.Module):
         log = logging.getLogger(__name__)
         if from_tf:
             raise NotImplementedError("TensorFlow checkpoints are not supported on this path (DESIGN.md section 7)")
-        if distill_config:
-            raise NotImplementedError("distillation is out of scope on this path (DESIGN.md section 7)")
         path = str(pretrained_model_name_or_path)
         if not os.path.exists(path):
             log.error("Model name '%s' was not found: pretrained model names need a download and there is no network on this path; "
@@ -667,6 +772,7 @@ class BertPreTrainedModel(nn.Module):
                     tar.extractall(tmp, filter="data")
                 root = tmp
             config = BertConfig.from_json_file(os.path.join(root, "bert_config.json"))
+            _apply_distill_config(config, distill_config, pooler)
             model = cls(config, *inputs, **kwargs)
             if state_dict is None:
                 state_dict = torch.load(os.path.join(root, "pytorch_model.bin"), map_location="cpu")
@@ -827,7 +933,7 @@ class BertModel(BertPreTrainedModel):
             raise L.DleError("pack_sequences and remove_padding are two different routes: turn one of them off")
         if self.encoder._checkpoint_activations:
             raise L.DleError("pack_sequences does not support activation checkpointing")
-        if not all(layer._fusable() for layer in self.encoder.layer):
+        if not all(layer._fusable() and not layer.distillation and not layer.attention.self.distillation for layer in self.encoder.layer):
             raise L.DleError("pack_sequences needs the fused layer (head size 64, gelu with bias, no distillation)")
         if S > 512 or S > self.config.max_position_embeddings:
             raise L.DleError(f"pack_sequences takes S <= 512 and S <= max_position_embeddings, got S = {S}")

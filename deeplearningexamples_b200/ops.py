@@ -291,6 +291,40 @@ class BertLayerFn(torch.autograd.Function):
 
 
 # -------------------------------------------------------------------------------------------------
+# the encoder layer of a distillation student or teacher: BertLayerFn that also hands out the layer's packed qkv [T, 3H] and attention
+# output att [T, H] (the states the reference caches at modeling.py:378-383) as autograd outputs, so that the distillation losses can
+# reach them.  Their incoming gradients fold into the layer backward: d att adds into the datt GEMM's epilogue (EPI_ADD) before the
+# attention backward, d qkv (Q and K columns) adds onto the attention backward's dqkv before the QKV dgrad, with its column sums
+# added to the q / k bias gradients.
+# -------------------------------------------------------------------------------------------------
+class BertLayerDistillFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, mask, wq, wk, wv, bq, bk, bv, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2, w_qkv, b_qkv, cfg):
+        B, S, A, p_attn, p_hid, eps, sid_attn, sid_h1, sid_h2, seq_first = cfg
+        ctx.cfg = cfg
+        ctx.set_materialize_grads(False)
+
+        def attn(qkv, seed_a, sdev):
+            return K.attn_fwd(qkv, mask, B, S, A, dropout_p=p_attn, seed=seed_a, dropout_stream=sid_attn, seq_first=seq_first, seed_dev=sdev)
+        states = []
+        y2 = _layer_forward(ctx, x, mask, attn, (wq, bq, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2), w_qkv, b_qkv, p_attn, p_hid, eps,
+                            sid_h1, sid_h2, states=states)
+        qkv, att = states
+        return y2, qkv, att
+
+    @staticmethod
+    def backward(ctx, dy2, dqkv_ext, datt_ext):
+        B, S, A, p_attn, p_hid, eps, sid_attn, sid_h1, sid_h2, seq_first = ctx.cfg
+
+        def attn_bwd(qkv, mask, att, datt, lse, seed_a, dbias, sdev):
+            return K.attn_bwd(qkv, mask, att, datt, lse, B, S, A, dropout_p=p_attn, seed=seed_a, dropout_stream=sid_attn,
+                              seq_first=seq_first, dbias=dbias, seed_dev=sdev)
+        if dy2 is None:                     # the layer output reaches no loss (the teacher's or a student's last layer)
+            dy2 = torch.zeros_like(ctx.saved_tensors[0])
+        return _layer_backward(ctx, dy2, attn_bwd, p_hid, sid_h1, sid_h2, dqkv_ext=dqkv_ext, datt_ext=datt_ext)
+
+
+# -------------------------------------------------------------------------------------------------
 # the encoder layer over packed tokens (BertModel.remove_padding in training): BertLayerFn with variable-length attention
 # -------------------------------------------------------------------------------------------------
 class BertLayerPackedFn(torch.autograd.Function):
@@ -321,9 +355,9 @@ class BertLayerPackedFn(torch.autograd.Function):
         return _layer_backward(ctx, dy2, attn_bwd, p_hid, sid_h1, sid_h2)
 
 
-def _layer_forward(ctx, x, attn_aux, attn, params, w_qkv, b_qkv, p_attn, p_hid, eps, sid_h1, sid_h2):
-    """Forward of BertLayerFn / BertLayerPackedFn.  attn(qkv, seed, seed_dev) -> (ctx, lse) is the layer's attention; attn_aux (mask
-    or cu_seqlens) is saved for its backward."""
+def _layer_forward(ctx, x, attn_aux, attn, params, w_qkv, b_qkv, p_attn, p_hid, eps, sid_h1, sid_h2, states=None):
+    """Forward of BertLayerFn / BertLayerPackedFn / BertLayerDistillFn.  attn(qkv, seed, seed_dev) -> (ctx, lse) is the layer's
+    attention; attn_aux (mask or cu_seqlens) is saved for its backward.  states: a list that receives (qkv, att), or None."""
     wq, bq, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2 = params
     seed_a = next_seed() if p_attn > 0.0 else 0
     seed_1 = next_seed() if p_hid > 0.0 else 0
@@ -339,13 +373,17 @@ def _layer_forward(ctx, x, attn_aux, attn, params, w_qkv, b_qkv, p_attn, p_hid, 
                 dropout_stream=sid_h2, seed_dev=sdev)
     y2, _, mean2, rstd2 = K.add_ln_fwd(z2, w16(g2), w16(be2), eps=eps)
     ctx.save_for_backward(x, attn_aux, qkv, att, lse, z1, mean1, rstd1, y1, u, g, z2, mean2, rstd2, w_qkv)
+    if states is not None:
+        states.extend((qkv, att))
     ctx.params = params
     ctx.seeds = (seed_a, seed_1, seed_2)
     return y2
 
 
-def _layer_backward(ctx, dy2, attn_bwd, p_hid, sid_h1, sid_h2):
-    """Backward of BertLayerFn / BertLayerPackedFn.  attn_bwd(qkv, attn_aux, ctx, dctx, lse, seed, dbias, seed_dev) -> dqkv."""
+def _layer_backward(ctx, dy2, attn_bwd, p_hid, sid_h1, sid_h2, dqkv_ext=None, datt_ext=None):
+    """Backward of BertLayerFn / BertLayerPackedFn / BertLayerDistillFn.  attn_bwd(qkv, attn_aux, ctx, dctx, lse, seed, dbias, seed_dev)
+    -> dqkv.  dqkv_ext / datt_ext: gradients that reach the layer's qkv (Q and K columns) and attention output from outside (the
+    distillation losses), or None."""
     x, attn_aux, qkv, att, lse, z1, mean1, rstd1, y1, u, g, z2, mean2, rstd2, w_qkv = ctx.saved_tensors
     wq, bq, wo, bo, g1, be1, w1, b1, w2, b2, g2, be2 = ctx.params
     seed_a, seed_1, seed_2 = ctx.seeds
@@ -366,10 +404,15 @@ def _layer_backward(ctx, dy2, attn_bwd, p_hid, sid_h1, sid_h2):
     # ---- BertSelfOutput
     dz1, dh1, dg1, dbe1, dbo = K.add_ln_bwd(dy1, z1, mean1, rstd1, w16(g1), dropout_p=p_hid, seed=seed_1, dropout_stream=sid_h1,
                                             out_dtype=g1.dtype, seed_dev=sdev)
-    datt = K.gemm(dh1, w16(wo), b_layout=L.LAYOUT_MN)
+    if datt_ext is None:
+        datt = K.gemm(dh1, w16(wo), b_layout=L.LAYOUT_MN)
+    else:
+        datt = K.gemm(dh1, w16(wo), b_layout=L.LAYOUT_MN, epilogue=L.EPI_ADD, aux=datt_ext.contiguous())
     dwo = wgrad(dh1, att, wo.dtype)
     # ---- BertSelfAttention (+ residual branch of BertSelfOutput folded into the QKV dgrad epilogue)
     dqkv = attn_bwd(qkv, attn_aux, att, datt, lse, seed_a, dbqkv_acc, sdev)
+    if dqkv_ext is not None:            # the loss's Q / K gradient, and its share of the q / k bias gradients
+        K.add_rows_bf16(dqkv[:, :2 * H_], dqkv_ext[:, :2 * H_], colsum=dbqkv_acc[:2 * H_])
     dx = K.gemm(dqkv, w16(w_qkv, key=wq), b_layout=L.LAYOUT_MN, epilogue=L.EPI_ADD, aux=dz1)
     dwqkv = wgrad(dqkv, x, wq.dtype)
     bias_g = bias_acc if b1.dtype == torch.float32 else bias_acc.to(b1.dtype)
@@ -529,3 +572,62 @@ class SoftmaxCrossEntropyFn(torch.autograd.Function):
         x, labels, lse, count = ctx.saved_tensors
         scale = (g.to(torch.float32) / count).reshape(1).contiguous()
         return K.softmax_ce_bwd(x, labels, lse, scale, ctx.ignore_index), None, None
+
+
+# -------------------------------------------------------------------------------------------------
+# distillation losses on the student / teacher states, without the [B, A, S, S] tensors
+# replaces TransformerLosses.compute_loss_ "kld" and "cosine" (distillation/losses.py:37-88)
+# -------------------------------------------------------------------------------------------------
+class RelationKLFn(torch.autograd.Function):
+    """loss = sum over the B*A*S query rows of KL(softmax(t) || softmax(s)) / (B*A*S) (KLDivLoss(batchmean) / (A*S)).
+    kind "attention": src = packed qkv [T, 3H]; s, t = Q K^T * scale + mask, then where(x <= -100, 0, x) (losses.py:80-85).
+    kind "value": src = attention output [T, H]; s, t = ctx ctx^T * scale per head (losses.py:41-61).
+    cfg = (kind, B, S, A, seq_first, mask_s, mask_t, scale_s, scale_t).  Only the student (src_s) gets a gradient."""
+
+    @staticmethod
+    def forward(ctx, src_s, src_t, cfg):
+        kind, B, S, A, seq_first, mask_s, mask_t, scale_s, scale_t = cfg
+        ops_s, ops_t = _relkl_operands(kind, src_s, A), _relkl_operands(kind, src_t, A)
+        norm = 1.0 / (B * A * S)
+        loss, lse_s, lse_t = K.relkl_fwd(*ops_s, *ops_t, mask_s, mask_t, B, S, A, scale_s, scale_t, kind == "attention", seq_first, norm)
+        ctx.save_for_backward(src_s, src_t, lse_s, lse_t)
+        ctx.cfg = cfg
+        return loss
+
+    @staticmethod
+    def backward(ctx, g):
+        src_s, src_t, lse_s, lse_t = ctx.saved_tensors
+        kind, B, S, A, seq_first, mask_s, mask_t, scale_s, scale_t = ctx.cfg
+        H = A * 64
+        d = torch.empty(src_s.shape, device=src_s.device, dtype=bf16)
+        if kind == "attention":
+            dx, dy, dzero = d[:, :H], d[:, H:2 * H], d[:, 2 * H:3 * H]
+        else:
+            dx, dy, dzero = d, d, None
+        K.relkl_bwd(*_relkl_operands(kind, src_s, A), *_relkl_operands(kind, src_t, A), mask_s, mask_t, B, S, A, scale_s, scale_t,
+                    kind == "attention", seq_first, lse_s, lse_t, g.to(torch.float32).reshape(1).contiguous(), 1.0 / (B * A * S),
+                    dx, dy, dzero)
+        return d, None, None
+
+
+def _relkl_operands(kind, src, A):
+    """(X, Y) head-0 column views of a packed qkv [T, 3H] (Q, K) or of an attention output [T, H] (ctx, ctx)."""
+    if kind == "attention":
+        H = A * 64
+        return src[:, :H], src[:, H:2 * H]
+    return src, src
+
+
+class CosineRowsFn(torch.autograd.Function):
+    """mean over rows of 1 - cos(pred_r, target_r): CosineEmbeddingLoss()(pred, target, 1) (losses.py:63-70); pred, target bf16
+    [rows, H].  Only pred gets a gradient."""
+
+    @staticmethod
+    def forward(ctx, pred, target):
+        ctx.save_for_backward(pred, target)
+        return K.cosine_rows_fwd(pred, target)
+
+    @staticmethod
+    def backward(ctx, g):
+        pred, target = ctx.saved_tensors
+        return K.cosine_rows_bwd(pred, target, g.to(torch.float32).reshape(1).contiguous()), None

@@ -320,6 +320,47 @@ int dle_adam_step(void* plan, const float* scale, float max_grad_norm, float cli
 /* standalone multi-tensor L2 norm over the plan's gradients (fused_lamb_CUDA.multi_tensor_l2norm) */
 int dle_lamb_grad_norm(void* plan, float* norm_out, float* found_inf_out, void* stream);
 
+/* ------------------------------------------------------------------------------------------
+ * General distillation losses (MiniLM / TinyBERT backbone distillation), without the [B, A, S, S] tensors.
+ *
+ * Relation-KL: per (b, h) the student logits s = scale_s * X_s Y_s^T (+ mask_s) and teacher logits t = scale_t * X_t Y_t^T (+ mask_t),
+ * each [S, S]; with where_rule != 0 every logit <= -100 (masked keys included) becomes 0 first.
+ *   loss = norm * sum over the B*A*S query rows of KL(softmax(t) || softmax(s))
+ * X / Y point at the 64 columns of head 0 in token-row matrices with row strides ld_s / ld_t (head h is 64*h columns further);
+ * token row of (b, s) = b*S + s, or s*B + b when seq_first.  Head dim 64, S % 64 == 0, S <= 512.
+ *   attention scores : X = Q, Y = K (column blocks 0 and A of the packed qkv), mask, where_rule = 1
+ *   value relation   : X = Y = ctx, no mask, where_rule = 0, scale = 1/sqrt(64)
+ * replaces: TransformerLosses.compute_loss / compute_loss_ with attention_loss = value_state_loss = "kld"
+ *   distillation/losses.py:37-61,77-88 (torch.where, bmm, LogSoftmax, Softmax, KLDivLoss(batchmean) / (A*S)) and the score tensor
+ *   modeling.py:298-300,378-383 it reads.
+ * fwd: lse_s / lse_t fp32 [B, A, S] for backward; partial fp32 [dle_relkl_partials(B, S, A)] workspace; loss fp32 [1].  Partials are
+ *   summed in a fixed order (no atomics): bitwise reproducible and graph-capturable.
+ * bwd: dS = grad_scale[0] * norm * scale_s * (p_s - p_t), 0 where the where rule substituted; dx = dS Y_s, dy = dS^T X_s (bf16, row
+ *   stride ld_d, head-0 column block).  dx == dy (X = Y) adds dS^T X_s onto dS Y_s.  dzero (or NULL): a head-0 column block that is
+ *   zero-filled (the V block of a packed qkv gradient). */
+int dle_relkl_partials(int32_t B, int32_t S, int32_t A);
+int dle_relkl_fwd(const void* xs, const void* ys, const void* xt, const void* yt, int64_t ld_s, int64_t ld_t, const float* mask_s,
+                  const float* mask_t, float scale_s, float scale_t, int32_t where_rule, int32_t B, int32_t S, int32_t A, int32_t seq_first,
+                  float norm, float* lse_s, float* lse_t, float* partial, float* loss, void* stream);
+int dle_relkl_bwd(const void* xs, const void* ys, const void* xt, const void* yt, int64_t ld_s, int64_t ld_t, const float* mask_s,
+                  const float* mask_t, float scale_s, float scale_t, int32_t where_rule, int32_t B, int32_t S, int32_t A, int32_t seq_first,
+                  const float* lse_s, const float* lse_t, const float* grad_scale, float norm, void* dx, void* dy, void* dzero,
+                  int64_t ld_d, void* stream);
+/* Cosine rows: loss = mean over rows of 1 - <x, y> / sqrt((|x|^2 + 1e-12)(|y|^2 + 1e-12)) on bf16 rows [rows, H], fp32 arithmetic.
+ * replaces: CosineEmbeddingLoss()(pred.view(-1, H), target.view(-1, H), 1), distillation/losses.py:63-70 (hidden / embedding states).
+ * fwd: partial fp32 [dle_cosine_rows_partials(rows)] workspace, loss fp32 [1], fixed-order sums.  bwd: dx (bf16) = grad_scale[0] *
+ * d loss / dx; no gradient for y (the teacher). */
+int dle_cosine_rows_partials(int64_t rows);
+int dle_cosine_rows_fwd(const void* x, int64_t ldx, const void* y, int64_t ldy, int64_t rows, int32_t H, float* partial, float* loss,
+                        void* stream);
+int dle_cosine_rows_bwd(const void* x, int64_t ldx, const void* y, int64_t ldy, int64_t rows, int32_t H, const float* grad_scale,
+                        void* dx, int64_t ldd, void* stream);
+/* dst[r, c] += src[r, c] on bf16 [rows, cols] (fp32 add, one rounding); colsum (fp32 [cols] or NULL) += column sums of src, atomics.
+ * Folds a distillation loss's gradient of an encoder layer's qkv into the layer's own before its QKV dgrad (the loss term of the
+ * q / k bias gradients, BertSelfAttention.query / key in modeling.py:298-300). */
+int dle_add_rows_bf16(void* dst, int64_t ld_dst, const void* src, int64_t ld_src, int64_t rows, int32_t cols, float* colsum,
+                      void* stream);
+
 #ifdef __cplusplus
 }
 #endif
